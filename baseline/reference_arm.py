@@ -3,29 +3,21 @@ from __future__ import annotations
 
 import json
 import os
-import shutil
 import sys
 import time
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REF_DIR = os.path.join(HERE, "_ref")
+REF_DIR = os.path.join(os.path.dirname(HERE), "oracle", "_ref")  # staged by build() (oracle/stage_reference.py)
 SHIMS = os.path.join(HERE, "shims")
-REF_SRC = "/root/reference"
 
 
 def _ensure_ref():
-    need = ["run_vit_training.py", "utils.py"]
-    if all(os.path.exists(os.path.join(REF_DIR, f)) for f in need):
+    if all(os.path.exists(os.path.join(REF_DIR, m + ".pyc")) for m in ("run_vit_training", "utils")):
         return None
-    if not os.path.isdir(REF_SRC):
-        return f"baseline/_ref is missing and {REF_SRC} is not available to copy it from"
-    os.makedirs(REF_DIR, exist_ok=True)
-    for f in need:
-        shutil.copy(os.path.join(REF_SRC, f), os.path.join(REF_DIR, f))
-    return None
+    return "the reference is not staged under oracle/_ref (build() stages it when the reference project is available)"
 
 
-def run(args, MODELS, ClockSampler, time_steps):
+def run(args, MODELS, ClockSampler, time_steps, model_depth):
     import torch
     import torch.distributed as dist
 
@@ -56,9 +48,7 @@ def run(args, MODELS, ClockSampler, time_steps):
     from vit_10b_fsdp_example_b200.config import parse_args  # flag-compatible argparse (same 29 flags/defaults)
 
     image, patch, dim, heads, blocks, mlp, desc = MODELS[args.model]
-    reduced = bool(args.num_blocks)
-    if reduced:
-        blocks = args.num_blocks
+    blocks, reduced = model_depth(args, world, dim, blocks)  # same depth as the other arm
     global_batch = args.local_batch * world
     cfg = parse_args(["--fake_data", "--image_size", str(image), "--patch_size", str(patch), "--embed_dim", str(dim),
                       "--num_heads", str(heads), "--num_blocks", str(blocks), "--mlp_ratio", str(mlp),

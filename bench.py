@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Headline benchmark: ViT-10B FSDP training throughput (images/sec) on N B200 GPUs of one node.
+"""Headline benchmark: ViT-10B FSDP training throughput (images/sec) on N H100 GPUs of one node.
 
     python bench.py                                   # 1 GPU, 5 timed steps, 3 warm-ups
+    python bench.py --dump-outputs DIR                # also write what the last timed step computed to DIR/*.npy
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus 8 --steps 5 --warmup 3
     python bench.py --impl reference ...              # the UNMODIFIED reference script on stock PyTorch
@@ -13,6 +14,9 @@ Protocol (BASELINE.md): ViT-10B (embed 5120, 32 heads, 32 blocks, MLP 4x, patch 
 `--fake_data` zeros, random-init weights, FSDP ZeRO-3 + activation checkpointing + grad clipping + AdamW +
 warmup-cosine -- the full training step of the reference.  Weak scaling: 128 images per GPU (= the
 reference's global batch 1024 on 8 GPUs).  Step time comes from CUDA events on the device, max over ranks.
+One 80 GB GPU cannot hold the model (AdamW state, fp32-exact weights and gradients take about 14 bytes per parameter,
+so 10 B parameters need ~140 GB): on a single GPU the same blocks are trained at depth ONE_GPU_BLOCKS and the result is
+marked as reduced.
 
 Two timed regions of K steps each:
   * e2e   : every step copies that step's batch from pinned host memory to the device and reads the loss back;
@@ -41,6 +45,19 @@ MODELS = {
     "vitb": (224, 16, 768, 12, 12, 4.0, "ViT-Base (debug)"),
 }
 
+# ViT-10B blocks (315 M parameters, ~4.4 GB of training state each) that fit one 80 GB GPU next to the activations of
+# 128 images; used when --gpus 1 runs a 32-block model and --num_blocks is not given.
+ONE_GPU_BLOCKS = 8
+
+
+def model_depth(args, world, dim, blocks):
+    """(blocks to train, whether that is fewer than the model has) -- the same for both arms."""
+    if args.num_blocks:
+        return args.num_blocks, True
+    if world == 1 and dim >= 5120 and blocks > ONE_GPU_BLOCKS:
+        return ONE_GPU_BLOCKS, True
+    return blocks, False
+
 
 def parse():
     ap = argparse.ArgumentParser()
@@ -50,7 +67,9 @@ def parse():
     ap.add_argument("--impl", type=str, default="ours", choices=["ours", "reference"])
     ap.add_argument("--model", type=str, default="vit10b", choices=sorted(MODELS))
     ap.add_argument("--local_batch", type=int, default=128)
-    ap.add_argument("--num_blocks", type=int, default=0, help="debug: override depth (marks the result as reduced)")
+    ap.add_argument("--num_blocks", type=int, default=0,
+                    help="override depth (marks the result as reduced); 0 = the model's depth, or ONE_GPU_BLOCKS "
+                         "for the 10 B models on a single GPU")
     ap.add_argument("--backend", type=str, default="sm100", choices=["sm100", "nccl"])
     ap.add_argument("--no_grad_ckpt", action="store_true")
     ap.add_argument("--ckpt_keep_blocks", type=int, default=-1,
@@ -61,6 +80,9 @@ def parse():
     ap.add_argument("--no_e2e", action="store_true")
     ap.add_argument("--cuda_graph", type=int, default=-1,
                     help="1/0: replay the training step as one CUDA graph; -1 = auto (on for launch-bound models)")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="after the timed steps write what the last timed step returned and left behind (loss, gradient "
+                         "norm, a fixed seeded sample of every unit's gradients and updated fp32 weights) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -154,6 +176,34 @@ def _time_steps(torch, dist, world, step_fn, steps):
     return float(ms.item())
 
 
+def _dump_outputs(torch, model, loss, out_dir, per_unit=65536):
+    """What the last timed step returned and left behind, as float32 ``.npy`` files:
+      loss.npy            the loss it returned;
+      grad_norm.npy       the global gradient norm it clipped with (absent when the step ran as a CUDA graph);
+      grads_sample.npy    per FSDP unit, `per_unit` entries of this rank's reduced gradient shard;
+      weights_sample.npy  the fp32 master weights at the same positions after the optimizer update.
+    Positions are drawn once from a fixed seed, units are concatenated in model order (34 units x 64 Ki floats = 9 MB
+    per file at full depth).  The learning rate is still in warm-up during a benchmark, so the weights barely move:
+    loss, norm and gradients are what tells two builds apart.  Inputs are identical from run to run; the bias
+    gradients are summed with fp32 atomics, so outputs repeat to about 1e-5 relative, not bit for bit."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    norm = getattr(model, "_grad_norm", None)
+    if norm is not None:
+        np.save(os.path.join(out_dir, "grad_norm.npy"), norm.detach().float().reshape(1).cpu().numpy())
+    gen = torch.Generator().manual_seed(0)
+    weights, grads = [], []
+    for unit in model.all_units:
+        w = model.master_fp32(unit)
+        idx = torch.randint(0, w.numel(), (min(per_unit, w.numel()),), generator=gen).to(w.device)
+        weights.append(w[idx].float().cpu())
+        grads.append(unit.shard_grad[idx].float().cpu())
+    np.save(os.path.join(out_dir, "weights_sample.npy"), torch.cat(weights).numpy())
+    np.save(os.path.join(out_dir, "grads_sample.npy"), torch.cat(grads).numpy())
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -174,9 +224,7 @@ def run_ours(args):
         dist.init_process_group("nccl", rank=rank, world_size=world, device_id=device)
 
     image, patch, dim, heads, blocks, mlp, desc = MODELS[args.model]
-    reduced = False
-    if args.num_blocks:
-        blocks, reduced = args.num_blocks, True
+    blocks, reduced = model_depth(args, world, dim, blocks)
     vcfg = ViTConfig(image_size=image, patch_size=patch, embed_dim=dim, num_heads=heads, num_blocks=blocks,
                      mlp_ratio=mlp, num_classes=1000)
     t_init = time.time()
@@ -222,8 +270,10 @@ def run_ours(args):
         loss = train_step(images, target)
         last_loss[0] = float(loss.item())  # device -> host read of the step's result (4 bytes)
 
+    dev_loss = [None]
+
     def step_dev():
-        train_step(dev_images, dev_target)
+        dev_loss[0] = train_step(dev_images, dev_target)
 
     for _ in range(max(args.warmup, 3) + (2 if use_graph else 0)):
         step_e2e()  # with --cuda_graph the first calls are eager warm-up + capture
@@ -236,13 +286,15 @@ def run_ours(args):
     n0 = cuda_ops.launch_count()
     dev_ms = _time_steps(torch, dist, world, step_dev, args.steps)
     launches = cuda_ops.launch_count() - n0
+    if args.dump_outputs and rank == 0:
+        _dump_outputs(torch, model, dev_loss[0], args.dump_outputs)
     if graphed is not None:  # kernels replayed from the graph never pass through the Python wrappers
         launches = graphed.launches_per_step * args.steps
     clocks = sampler.stop() if sampler else {}
     peak_gb = torch.cuda.max_memory_allocated() / 1e9
     exposed = None
     if graphed is None:
-        # Secondary metric of BASELINE.json: exposed communication per step, probed outside the timed region.
+        # Secondary metric of BASELINE.md: exposed communication per step, probed outside the timed region.
         # A rank that is ahead of its peers also waits for *them* inside these events (GPUs under a power cap run at
         # different clocks), so the rank with the smallest stall is the critical path: its number is the exposed
         # communication; the largest one mostly measures how unequal the GPUs are.
@@ -290,7 +342,7 @@ def run_ours(args):
                                            f"outputs / gelu(u)), {blocks - kept} are recomputed in backward"),
                        "optimizer": "AdamW + clip_grad_norm 1.0 + warmup-cosine, every step",
                        "cuda_graph": bool(use_graph),
-                       "l2": "no explicit flush: each step streams ~20 GB of bf16 weights plus activations (>> 126 MB L2)",
+                       "l2": "no explicit flush: each step streams ~20 GB of bf16 weights plus activations (>> 50 MB L2)",
                        "params": vcfg.total_numel()},
             "clocks": {"sm_mhz": clocks.get("sm_mhz"), "sm_max_mhz": clocks.get("sm_max_mhz"),
                        "reasons": clocks.get("reasons", []), "samples": clocks.get("samples", 0),
@@ -320,7 +372,7 @@ def run_reference(args):
     except Exception as e:  # pragma: no cover
         print(json.dumps({"impl": "reference", "unavailable": f"reference arm not importable: {e!r}"[:300]}))
         return
-    reference_arm.run(args, MODELS, ClockSampler, _time_steps)
+    reference_arm.run(args, MODELS, ClockSampler, _time_steps, model_depth)
 
 
 def main():

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""ViT-10B FSDP training on B200 -- flag-compatible entry point.
+"""ViT-10B FSDP training on H100 -- flag-compatible entry point.
 
 Accepts the reference's command line unchanged (run_vit_training.py:327-363), e.g.
 

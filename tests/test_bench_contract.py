@@ -1,4 +1,4 @@
-"""bench.py's contract with the driver, as far as a CPU box can check it: flags and defaults, the clock / throttle
+"""bench.py's command-line contract, as far as a machine without a GPU can check it: flags and defaults, the clock / throttle
 sampler, the keys of the JSON line, and the reference arm's 'always one JSON line, exit 0' rule."""
 import json
 import os
@@ -9,6 +9,7 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_flags_and_defaults(monkeypatch):
@@ -22,7 +23,39 @@ def test_flags_and_defaults(monkeypatch):
     a = bench.parse()
     assert (a.gpus, a.steps, a.warmup, a.impl) == (8, 20, 5, "reference")
     img, patch, dim, heads, blocks, ratio, _ = bench.MODELS["vit10b"]
-    assert (img, patch, dim, heads, blocks, ratio) == (224, 14, 5120, 32, 32, 4.0)   # BASELINE.json's headline config
+    assert (img, patch, dim, heads, blocks, ratio) == (224, 14, 5120, 32, 32, 4.0)   # BASELINE.md's headline config
+    assert 1 <= bench.ONE_GPU_BLOCKS < blocks and a.num_blocks == 0     # depth one 80 GB GPU holds; --num_blocks overrides
+    monkeypatch.setattr(sys, "argv", ["bench.py", "--steps", "2", "--dump-outputs", "/tmp/x"])
+    a = bench.parse()
+    assert a.steps == 2 and a.dump_outputs == "/tmp/x"
+
+
+def test_dump_outputs_writes_loss_norm_and_seeded_samples(tmp_path):
+    """One CPU training step of a tiny model, then the dump: float32 arrays, same positions on every call."""
+    import numpy as np
+    import torch
+
+    import bench
+    from helpers import tiny_cfg
+    from vit_10b_fsdp_example_b200.parallel import FSDPViT, ShardedAdamW
+
+    cfg = tiny_cfg()
+    model = FSDPViT(cfg, dtype=torch.float32, seed=0)
+    opt = ShardedAdamW(model, lr=1e-3, weight_decay=0.1)
+    images = torch.zeros(2, 3, cfg.image_size, cfg.image_size)
+    loss = model.forward_backward(images, torch.zeros(2, dtype=torch.long))
+    norm = model.clip_grad_norm_(1.0)
+    opt.step()
+    bench._dump_outputs(torch, model, loss, str(tmp_path / "a"), per_unit=100)
+    bench._dump_outputs(torch, model, loss, str(tmp_path / "b"), per_unit=100)
+    got = {n: np.load(tmp_path / "a" / f"{n}.npy") for n in ("loss", "grad_norm", "grads_sample", "weights_sample")}
+    assert all(v.dtype == np.float32 for v in got.values())
+    assert got["loss"][0] == np.float32(loss.item()) and got["grad_norm"][0] == np.float32(norm.item())
+    n = sum(min(100, u.layout.shard_numel) for u in model.all_units)
+    assert got["weights_sample"].shape == got["grads_sample"].shape == (n,)
+    assert np.abs(got["grads_sample"]).max() > 0 and np.isfinite(got["weights_sample"]).all()
+    for name, arr in got.items():
+        assert np.array_equal(arr, np.load(tmp_path / "b" / f"{name}.npy")), name
 
 
 def test_clock_sampler_parses_nvidia_smi_rows(tmp_path, monkeypatch):
@@ -58,8 +91,8 @@ def test_json_line_has_every_key_the_driver_reads():
 
 
 def test_reference_arm_always_prints_one_json_line_and_exits_zero():
-    """On this GPU-less box the reference cannot run: the arm must still exit 0 with {"impl": "reference",
-    "unavailable": ...} (the driver's rule for an arm that cannot be measured)."""
+    """Without a GPU the reference cannot run: the arm must still exit 0 with {"impl": "reference",
+    "unavailable": ...} (the rule for an arm that cannot be measured)."""
     r = subprocess.run([sys.executable, "bench.py", "--impl", "reference", "--steps", "1", "--warmup", "1"], cwd=ROOT,
                        capture_output=True, text=True, timeout=300, env=dict(os.environ, CUDA_VISIBLE_DEVICES=""))
     assert r.returncode == 0, r.stderr[-2000:]

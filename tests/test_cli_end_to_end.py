@@ -1,4 +1,4 @@
-"""The flag-compatible entry point end to end on CPU/gloo (BASELINE.json config 1: ViT-Tiny-like, W=2, --fake_data):
+"""The flag-compatible entry point end to end on CPU/gloo (BASELINE.md's plumbing config: ViT-Tiny-like, W=2, --fake_data):
 train -> per-rank checkpoints -> resume -> evaluate -> offline consolidation, all through the command line."""
 import os
 import subprocess
@@ -150,7 +150,7 @@ def test_every_strategy_flag_through_the_cli_gives_the_same_trajectory(tmp_path)
 
 
 def test_a_dying_rank_takes_the_job_down_and_resume_continues(tmp_path):
-    """Failure contract (SURVEY 5.3): a rank that crashes mid-epoch must not leave its peers hanging in a collective --
+    """Failure contract: a rank that crashes mid-epoch must not leave its peers hanging in a collective --
     the launcher exits non-zero in bounded time -- and the run continues from the last checkpoint with --resume_epoch."""
     ckpt = str(tmp_path / "ckpt")
     ok = _run(["run_vit_training.py", *TINY, "--ckpt_dir", ckpt, "--num_epochs", "1"])

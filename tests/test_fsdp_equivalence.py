@@ -1,4 +1,4 @@
-"""Equivalence matrix (SURVEY §4.2): every sharding / scheduling flag must leave the numerics unchanged.
+"""Equivalence matrix: every sharding / scheduling flag must leave the numerics unchanged.
 
 FSDP (W=1,2,4) x --run_without_fsdp x grad-ckpt x reshard x flatten x shard_on_cpu all have to produce the
 same loss / grad-norm trajectory as the single-process run on the same global batch.

@@ -1,4 +1,4 @@
-"""Memory-bound sm_100a kernels vs the fp32 PyTorch reference ops."""
+"""Memory-bound sm_90a kernels vs the fp32 PyTorch reference ops."""
 import os
 import sys
 

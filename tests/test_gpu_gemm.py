@@ -1,4 +1,4 @@
-"""tcgen05 GEMM vs an fp32 PyTorch reference (all operand majors, tile widths, fused epilogues)."""
+"""wgmma GEMM vs an fp32 PyTorch reference (all operand majors, tile widths, fused epilogues)."""
 import os
 import sys
 

@@ -40,7 +40,7 @@ def test_vit10b_block_layout_numbers():
     from vit_10b_fsdp_example_b200.models import vit
 
     cfg = ViTConfig()
-    assert cfg.block_numel() == 314_639_360           # SURVEY §6.2
+    assert cfg.block_numel() == 314_639_360
     assert cfg.total_numel() == 10_077_917_160        # "10 billion parameters"
     lay = UnitLayout.build("blocks.0", vit.block_param_specs(cfg), 8, False)
     assert lay.payload_numel() == cfg.block_numel()

@@ -58,7 +58,7 @@ def test_injected_faults_are_detected(bug, args):
 def test_forward_softmax_to_epilogue_handoff_needs_its_mbarrier():
     """Round-2 forward: 1 / row sum travels from the softmax warps to the separate epilogue warps through a plain
     shared-memory slot ordered only by the stat_full mbarrier (the pair compute-sanitizer racecheck flags, see
-    profiles/r2_sanitizer.md).  With the wait the protocol holds for every schedule; without it the model must see
+    of the kernel tests).  With the wait the protocol holds for every schedule; without it the model must see
     the epilogue read a slot that is stale or half written."""
     for seed in range(120):
         pm.model_fwd_persist(seed, 5, 4)

@@ -320,7 +320,7 @@ def model_fwd_persist(seed: int, n_items: int, nkt: int, warps: int = 4, bug: st
     """Round-2 kernel: 4 softmax warps (row max, exp2, P ring, 1/sum into s_inv[item & 1]) and 4 separate epilogue
     warps (wait stat_full[item & 1] -> read s_inv -> wait acc_full -> read O -> arrive acc_empty).  The s_inv slot is a
     plain shared-memory hand-off between generic-proxy threads ordered ONLY by the stat_full mbarrier -- the pair
-    compute-sanitizer racecheck reports (profiles/r2_sanitizer.md).  bug="no_stat_full" drops that wait (the model must
+    compute-sanitizer racecheck reports.  bug="no_stat_full" drops that wait (the model must
     then see the epilogue read a stale / half-written slot); bug="stat_single" uses one slot instead of two."""
     s = Sim(seed)
     W = warps

@@ -1,11 +1,11 @@
-"""Per-kernel SASS mnemonic census (proof of tcgen05 / TMA / multimem use) -> profiles/sass_summary.md"""
+"""Per-kernel SASS mnemonic census (proof of wgmma / TMA / multimem use), printed or written as markdown."""
 import collections
 import re
 import subprocess
 import sys
 
-OBJS = ["gemm_sm100.cu.o", "attention_sm100.cu.o", "attention_bwd_sm100.cu.o", "attention_persist_sm100.cu.o", "attention_bwd_persist_sm100.cu.o", "comm.cu.o", "elementwise.cu.o", "layernorm_stream.cu.o"]
-INTEREST = re.compile(r"^(UTCHMMA|UTCQMMA|UTMALDG|UTMASTG|UBLKCP|LDTM|STTM|UTCBAR|UTCATOMSWS|UTCCP|SYNCS|MULTIMEM|"
+OBJS = ["gemm_sm90.cu.o", "attention_sm90.cu.o", "comm.cu.o", "elementwise.cu.o", "layernorm_stream.cu.o"]
+INTEREST = re.compile(r"^(HGMMA|WARPGROUP|UTMALDG|UTMASTG|UBLKCP|SYNCS|MULTIMEM|"
                       r"LDGMC|LDG\.E\.NA|STG\.E\.NA|LDG\.E\.STRONG|STG\.E\.STRONG|LDG\.E\.128|STG\.E\.128|RED|ATOM|MEMBAR|HMMA|UCGABAR)")
 
 
@@ -37,9 +37,10 @@ def census(build_dir, objs=None):
 
 
 def main(build_dir, out):
-    lines = ["# SASS census of the hand-written kernels (cuobjdump -sass, sm_100a)", "",
-             "`UTCHMMA` = tcgen05.mma, `UTMALDG/UTMASTG` = TMA tensor load/store, `LDTM` = tcgen05.ld, `UTCBAR` = "
-             "tcgen05.commit, `UTCATOMSWS` = TMEM alloc, `SYNCS.*` = mbarrier, `LDGMC...HPADD` = multimem.ld_reduce (NVLS in-switch reduce), `LDG.E.NA.128` = streaming peer loads, `*.STRONG.SYS` = cross-GPU flags.", ""]
+    lines = ["# SASS census of the hand-written kernels (cuobjdump -sass, sm_90a)", "",
+             "`HGMMA` = wgmma.mma_async, `WARPGROUP.*` = wgmma fence / commit / wait, `UTMALDG/UTMASTG` = TMA tensor "
+             "load/store, `SYNCS.*` = mbarrier, `LDGMC...F32ADD` = multimem.ld_reduce (NVLS in-switch reduce), "
+             "`LDG.E.NA.128` = streaming peer loads, `*.STRONG.SYS` = cross-GPU flags.", ""]
     for obj, counts in census(build_dir).items():
         lines.append(f"## {obj}")
         lines.append("")
@@ -54,4 +55,4 @@ def main(build_dir, out):
 
 if __name__ == "__main__":
     main(sys.argv[1] if len(sys.argv) > 1 else "vit_10b_fsdp_example_b200/csrc/build",
-         sys.argv[2] if len(sys.argv) > 2 else "profiles/sass_summary.md")
+         sys.argv[2] if len(sys.argv) > 2 else "sass_summary.md")

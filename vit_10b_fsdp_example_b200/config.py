@@ -1,7 +1,7 @@
 """Command-line / configuration surface.
 
 The 29 flags of the reference (run_vit_training.py:327-363) are accepted verbatim with the same
-defaults (ViT-10B recipe).  B200-specific extras are optional and default to reference behaviour.
+defaults (ViT-10B recipe).  H100-specific extras are optional and default to reference behaviour.
 """
 from __future__ import annotations
 
@@ -10,7 +10,7 @@ from dataclasses import dataclass
 
 
 def build_arg_parser() -> argparse.ArgumentParser:
-    parser = argparse.ArgumentParser(description="B200-native FSDP ViT training")
+    parser = argparse.ArgumentParser(description="H100-native FSDP ViT training")
     # ---- reference flags (run_vit_training.py:329-336) ----
     parser.add_argument("--data_dir", type=str, default="/datasets/imagenet-1k")
     parser.add_argument("--fake_data", action="store_true", dest="fake_data")
@@ -43,7 +43,7 @@ def build_arg_parser() -> argparse.ArgumentParser:
     parser.add_argument("--flatten_parameters", action="store_true", dest="flatten_parameters")
     parser.add_argument("--run_without_fsdp", action="store_true", dest="run_without_fsdp")
     parser.add_argument("--shard_on_cpu", action="store_true", dest="shard_on_cpu")
-    # ---- B200 extras (not in the reference; defaults keep reference semantics) ----
+    # ---- H100 extras (not in the reference; defaults keep reference semantics) ----
     parser.add_argument("--init_from_full_ckpt", type=str, default="",
                         help="initialise the parameters from a consolidated (unsharded) checkpoint written by "
                              "consolidate_sharded_ckpts: continues a run on a different number of GPUs "

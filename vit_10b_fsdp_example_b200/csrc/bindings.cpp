@@ -1,4 +1,4 @@
-// pybind11 / ATen bindings for the sm_100a kernels.  Compiled by g++ (no CUDA device code here), so the
+// pybind11 / ATen bindings for the sm_90a kernels.  Compiled by g++ (no CUDA device code here), so the
 // .cu files stay free of the heavy torch headers and rebuild in seconds.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
@@ -8,10 +8,10 @@
 #include <optional>
 #include <vector>
 
-#include "attention_sm100.h"
+#include "attention_sm90.h"
 #include "comm.h"
 #include "elementwise.h"
-#include "gemm_sm100.h"
+#include "gemm_sm90.h"
 
 namespace {
 
@@ -99,69 +99,28 @@ void softmax_bwd(Tensor dp, Tensor p, int64_t rows, int64_t n, int64_t ld, doubl
     b200::softmax_bwd(bf16_mut(dp), bf16_ptr(p), rows, (int)n, ld, (float)scale, cur_stream());
 }
 
-bool attention_fwd_supported(int64_t N, int64_t hd) { return b200::attention_fwd_supported((int)N, (int)hd); }
+bool attention_supported(int64_t N, int64_t hd) { return b200::attention_supported((int)N, (int)hd); }
 
 void attention_fwd(Tensor qkv, Tensor out, OptT lse, OptT probs, int64_t B, int64_t N, int64_t H, int64_t hd) {
     c10::cuda::CUDAGuard guard(qkv.device());
     TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && out.is_contiguous(), "attention_fwd: bad layouts");
+    TORCH_CHECK(!lse.has_value() || (lse->is_contiguous() && lse->numel() == B * H * N), "attention_fwd: bad lse");
     b200::attention_fwd(bf16_ptr(qkv), qkv.stride(0), bf16_mut(out), lse.has_value() ? f32_ptr(*lse) : nullptr,
                         probs.has_value() ? bf16_mut(*probs) : nullptr, probs.has_value() ? probs->size(2) : 0, (int)B,
                         (int)N, (int)H, (int)hd, cur_stream());
 }
 
-void attention_fwd_long(Tensor qkv, Tensor out, Tensor lse, int64_t B, int64_t N, int64_t H, int64_t hd) {
-    c10::cuda::CUDAGuard guard(qkv.device());
-    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && out.is_contiguous() && lse.is_contiguous() &&
-                    lse.numel() == B * H * N,
-                "attention_fwd_long: bad layouts");
-    b200::attention_fwd_long(bf16_ptr(qkv), qkv.stride(0), bf16_mut(out), f32_ptr(lse), (int)B, (int)N, (int)H, (int)hd,
-                             cur_stream());
-}
-
-bool attention_fwd_persist_supported(int64_t N, int64_t hd) {
-    return b200::attention_fwd_persist_supported((int)N, (int)hd);
-}
-
-bool attention_fwd_long_supported(int64_t N, int64_t hd) {
-    return b200::attention_fwd_long_supported((int)N, (int)hd);
-}
-void attention_set_trace(OptT buf) {
-    if (!buf.has_value()) {
-        b200::attention_set_trace(nullptr, 0);
-        return;
-    }
-    TORCH_CHECK(buf->is_cuda() && buf->scalar_type() == at::kLong && buf->is_contiguous(), "trace: CUDA int64 tensor");
-    b200::attention_set_trace(reinterpret_cast<long long*>(buf->data_ptr()), (int)(buf->numel() / 16));
-}
-void attention_bwd_set_trace(OptT buf, int64_t role) {
-    if (!buf.has_value()) {
-        b200::attention_bwd_set_trace(nullptr, 0, 0);
-        return;
-    }
-    TORCH_CHECK(buf->is_cuda() && buf->scalar_type() == at::kLong && buf->is_contiguous(), "trace: CUDA int64 tensor");
-    b200::attention_bwd_set_trace(reinterpret_cast<long long*>(buf->data_ptr()), (int)(buf->numel() / 16), (int)role);
-}
-void attention_fwd_persist(Tensor qkv, Tensor out, OptT lse, int64_t B, int64_t N, int64_t H, int64_t hd) {
-    c10::cuda::CUDAGuard guard(qkv.device());
-    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && out.is_contiguous(), "attention_fwd_persist: bad layouts");
-    b200::attention_fwd_persist(bf16_ptr(qkv), qkv.stride(0), bf16_mut(out), lse.has_value() ? f32_ptr(*lse) : nullptr,
-                                (int)B, (int)N, (int)H, (int)hd, cur_stream());
-}
-
-bool attention_bwd_supported(int64_t N, int64_t hd) { return b200::attention_bwd_supported((int)N, (int)hd); }
-
 void attention_bwd(Tensor qkv, Tensor dout, Tensor out, Tensor lse, Tensor delta, Tensor dqkv, OptT colsum, int64_t B,
-                   int64_t N, int64_t H, int64_t hd, bool persist) {
+                   int64_t N, int64_t H, int64_t hd) {
     c10::cuda::CUDAGuard guard(qkv.device());
     TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && dout.stride(1) == 1 && out.stride(1) == 1 &&
                     dqkv.is_contiguous() && lse.is_contiguous() && delta.is_contiguous(),
                 "attention_bwd: bad layouts");
-    TORCH_CHECK(lse.numel() == B * H * N && delta.numel() == (persist ? 2 : 1) * B * H * N && dqkv.size(1) == 3 * H * hd,
-                "attention_bwd: bad shapes (delta needs two [B*H, N] planes for the persistent kernels)");
-    TORCH_CHECK(!persist || N % 4 == 0, "attention_bwd: persistent kernels need N % 4 == 0");
+    TORCH_CHECK(lse.numel() == B * H * N && delta.numel() == B * H * N && dqkv.size(1) == 3 * H * hd,
+                "attention_bwd: bad shapes");
     b200::attention_bwd(bf16_ptr(qkv), qkv.stride(0), bf16_ptr(dout), dout.stride(0), bf16_ptr(out), out.stride(0),
                         f32_ptr(lse), f32_ptr(delta), bf16_mut(dqkv), (int)B, (int)N, (int)H, (int)hd, cur_stream(),
-                        persist, colsum.has_value() ? f32_ptr(*colsum) : nullptr);
+                        colsum.has_value() ? f32_ptr(*colsum) : nullptr);
 }
 
 void cross_entropy(Tensor logits, Tensor target, OptT dlogits, Tensor loss, OptT correct) {
@@ -269,8 +228,8 @@ void p2p_all_gather(std::vector<int64_t> peer_ptrs, int64_t rank, Tensor out, Te
 }
 // Copy-engine transport of the all-gather: one asynchronous device-to-device copy per (parameter group, source rank)
 // straight from the peer's symmetric shard into its final place in the gathered buffer.  No SM, no shared memory, no
-// registers are taken from the GEMM running next to it, and the DMA engines keep the NVLink pipe full where SM-issued
-// peer loads do not (63 GB/s at W = 4 for the pull kernel, profiles/r2_n4.md).  Graph-capturable (memcpy nodes).
+// registers are taken from the GEMM running next to it.  Graph-capturable (memcpy nodes).  Its rate against the pull
+// kernel has not been measured on H100.
 void ce_all_gather(std::vector<int64_t> src_ptrs, std::vector<int64_t> dst_ptrs, std::vector<int64_t> nbytes) {
     TORCH_CHECK(src_ptrs.size() == dst_ptrs.size() && src_ptrs.size() == nbytes.size(), "ce_all_gather: ragged lists");
     cudaStream_t stream = cur_stream();
@@ -354,22 +313,15 @@ int64_t rs_chunk_vecs() { return b200::rs_chunk_vecs(); }
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-    m.doc() = "vit_10b_fsdp_example_b200 native sm_100a kernels";
+    m.doc() = "vit_10b_fsdp_example_b200 native sm_90a kernels";
     m.def("gemm", &gemm);
     m.def("layernorm_fwd", &layernorm_fwd);
     m.def("layernorm_bwd", &layernorm_bwd);
     m.def("softmax_fwd", &softmax_fwd);
     m.def("softmax_bwd", &softmax_bwd);
     m.def("attention_fwd", &attention_fwd);
-    m.def("attention_fwd_supported", &attention_fwd_supported);
-    m.def("attention_fwd_long", &attention_fwd_long);
-    m.def("attention_fwd_long_supported", &attention_fwd_long_supported);
-    m.def("attention_fwd_persist", &attention_fwd_persist);
-    m.def("attention_set_trace", &attention_set_trace);
-    m.def("attention_bwd_set_trace", &attention_bwd_set_trace);
-    m.def("attention_fwd_persist_supported", &attention_fwd_persist_supported);
+    m.def("attention_supported", &attention_supported);
     m.def("attention_bwd", &attention_bwd);
-    m.def("attention_bwd_supported", &attention_bwd_supported);
     m.def("cross_entropy", &cross_entropy);
     m.def("im2col", &im2col);
     m.def("gelu_fwd", &gelu_fwd);

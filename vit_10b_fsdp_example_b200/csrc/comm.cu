@@ -1,12 +1,11 @@
-// NVLink 5 / NVSwitch collectives over symmetric (peer-mapped) memory, written directly against raw
+// NVLink / NVSwitch collectives over symmetric (peer-mapped) memory, written directly against raw
 // peer / multicast pointers -- no NCCL on these paths.
 //
-// Design rule (measured, profiles/r2_timeline.md): a tcgen05 GEMM CTA owns 224 KB of shared memory and ~52 K
-// registers of its SM, so a 512-thread collective CTA cannot share an SM with it -- 24 such CTAs took 24 TPCs
-// (48 SMs) away from the 2-CTA GEMM clusters whenever a collective ran (+7 % step time from N = 2 on).  Every
-// kernel here is therefore a *light* CTA: 128 threads, <= 64 registers (8 K of the 13 K a GEMM CTA leaves free),
-// no shared memory, many 16-byte requests in flight per thread, and one such CTA on as many SMs as needed.  They
-// run *next to* the GEMM CTAs instead of instead of them.
+// Every kernel here is a *light* CTA: 128 threads, <= 96 registers, no shared memory, many 16-byte requests in
+// flight per thread, so that several fit one SM and a collective needs few SMs.  A resident GEMM CTA (gemm_sm90.cu)
+// takes 224 KB of shared memory and 384 x 168 of the SM's 65536 registers, so a collective CTA never shares an SM
+// with it: it is placed on an SM as a GEMM CTA retires.  How much of a collective hides under the GEMMs on H100 has
+// not been measured.
 //
 //   p2p_all_gather      : sync-free pull of the peers' parameter shards straight into their final
 //                         position in the gathered flat buffer (no copy-out pass).  Shards only change in

@@ -1,4 +1,4 @@
-// Memory-bound sm_100a kernels of the ViT training step: LayerNorm fwd/bwd, row softmax fwd/bwd,
+// Memory-bound sm_90a kernels of the ViT training step: LayerNorm fwd/bwd, row softmax fwd/bwd,
 // fused cross-entropy (loss + dlogits), patch im2col, bias-gradient column sums, sum of squares
 // (grad-norm partials) and the fused sharded AdamW update.
 //
@@ -259,7 +259,7 @@ __global__ void __launch_bounds__(kLnThreads, 3) ln_bwd_kernel(const __nv_bfloat
 // LayerNorm for narrow rows (D <= 2048): a row is handled by TPR threads (one 16 B vector each), a 256-thread CTA
 // works on 256/TPR rows at once, and a thread keeps the column accumulators of its 8 columns in registers.
 // The wide-row kernels above keep one row per CTA, which leaves most threads idle and serialises on two block
-// barriers per row when D is only 1024 (ViT-L): 136 us -> memory-bound.
+// barriers per row when D is only 1024 (ViT-L).
 // ------------------------------------------------------------------------------------------------
 template <int TPR>
 __device__ __forceinline__ void group_sum2(float& a, float& b, float* red, int row_slot) {

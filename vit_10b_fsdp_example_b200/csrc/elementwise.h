@@ -1,4 +1,4 @@
-// Host API of the memory-bound sm_100a kernels (see elementwise.cu).
+// Host API of the memory-bound sm_90a kernels (see elementwise.cu).
 // LayerNorm, softmax, GELU, cross-entropy, AdamW, clipping: the ATen/XLA ops behind run_vit_training.py:134-162,229,237,270.
 #pragma once
 #include <cuda_runtime.h>

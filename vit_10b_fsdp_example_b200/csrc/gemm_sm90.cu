@@ -1,0 +1,581 @@
+// Persistent, warp-specialised bf16 GEMM for sm_90a (H100):
+//   TMA (cp.async.bulk.tensor, SWIZZLE_128B)  ->  shared-memory ring (mbarrier full / empty pairs)
+//   wgmma.mma_async m64 x BLOCK_N x 16, two consumer warpgroups per CTA, fp32 accumulators in registers
+//   fused epilogue (bias, exact GELU, dGELU, residual add, pre-activation side output,
+//   bias-gradient column sums)  ->  swizzled smem  ->  TMA store.
+//
+// One CTA owns a 128 x BLOCK_N output tile; a producer warp (with a reduced register budget) keeps the ring
+// full while the consumer warpgroups (each 64 rows of the tile) issue the MMAs and run the epilogue.
+//
+//   D[b][m, n] = epilogue( sum_k A[b][m, k] * B[b][n, k] )
+//
+// A and B may each be K-major (reduction dim contiguous) or MN-major (reduction dim strided), which
+// covers forward (NT), dgrad (NN) and wgrad (TN) without materialising transposes.  Operands are 4-D
+// TMA tensors (inner, outer, batch_inner, batch_outer) so strided per-head attention operands inside a
+// packed qkv buffer are addressed in place.
+//
+// Capability parity: replaces the XLA-lowered dot ops under timm's Linear layers that the reference
+// calls at run_vit_training.py:134-141,153 (qkv / proj / fc1 / fc2 / head) and their autograd
+// backward.
+#include <cuda.h>
+#include <cuda_runtime.h>
+#include <cuda_bf16.h>
+#include <cstdint>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <mutex>
+#include <stdexcept>
+#include <string>
+#include <algorithm>
+#include <unordered_map>
+
+#include "gemm_sm90.h"
+#include "ptx.cuh"
+#include "wgmma.cuh"
+
+namespace b200 {
+
+namespace {
+
+constexpr int kBlockM = 128;  // rows per CTA: 64 per consumer warpgroup
+constexpr int kBlockK = 64;   // 64 bf16 = 128 B = one swizzle atom
+constexpr int kMmaK = 16;
+constexpr int kConsumerWgs = 2;
+constexpr int kNumThreads = 384;  // warpgroup 0: warp0 TMA producer, warp1 AG copier; warpgroups 1-2: wgmma + epilogue
+constexpr int kEpiThreads = 128;
+constexpr int kCdBufs = 4;            // two 64x64 bf16 staging buffers per consumer warpgroup for TMA stores
+constexpr int kCdBufBytes = 64 * 128;  // 64 rows x 128 B
+
+struct KernelParams {
+    int M, N, K;
+    int batch, nb_inner;
+    int m_tiles, n_tiles;  // CTA tiles (128 x BLOCK_N)
+    int n_rot;             // n-tile rotation so that tiles are visited in slab-arrival order (AG fusion)
+    int group_n;           // n-tiles per raster group
+    GemmEpilogue epi;
+    GemmAgFuse ag;
+};
+
+constexpr int kAgChunkBytes = 16384;
+
+__device__ __forceinline__ uint4 ld_peer_v4(const void* ptr) {
+    uint4 r;
+    asm volatile("ld.global.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+                 : "l"(ptr)
+                 : "memory");
+    return r;
+}
+__device__ __forceinline__ void red_release_gpu_add(uint32_t* ptr, uint32_t v) {
+    asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(ptr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* ptr) {
+    uint32_t v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ptr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
+
+// erf via Abramowitz-Stegun 7.1.26 (|err| < 1.5e-7, far below bf16 resolution): 1 rcp + 1 exp + 6 FMA.
+// e = exp(-z^2) is returned too: for z = x/sqrt(2) it is exactly the Gaussian factor gelu'(x) needs.
+__device__ __forceinline__ float erf_as(float z, float& e) {
+    const float az = fabsf(z);
+    const float t = __frcp_rn(fmaf(0.3275911f, az, 1.0f));
+    e = __expf(-az * az);
+    float poly = fmaf(1.061405429f, t, -1.453152027f);
+    poly = fmaf(poly, t, 1.421413741f);
+    poly = fmaf(poly, t, -0.284496736f);
+    poly = fmaf(poly, t, 0.254829592f);
+    const float y = 1.0f - poly * t * e;
+    return copysignf(y, z);
+}
+__device__ __forceinline__ float gelu_erf(float x) {
+    float e;
+    return 0.5f * x * (1.0f + erf_as(x * 0.70710678118654752f, e));
+}
+__device__ __forceinline__ float dgelu_erf(float x) {
+    float e;
+    const float cdf = 0.5f * (1.0f + erf_as(x * 0.70710678118654752f, e));
+    return fmaf(x * 0.3989422804014327f, e, cdf);  // cdf + x * pdf,  pdf = exp(-x^2/2)/sqrt(2 pi)
+}
+
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages>
+__global__ void __launch_bounds__(kNumThreads, 1)
+    gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                          const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_aux,
+                          const KernelParams p) {
+    constexpr int kABytes = kBlockM * kBlockK * 2;
+    constexpr int kBBytes = BLOCK_N * kBlockK * 2;
+    constexpr int kStageBytes = kABytes + kBBytes;
+    static_assert(BLOCK_N % 64 == 0 && BLOCK_N <= 256, "epilogue works in 64-column chunks; wgmma N <= 256");
+    static_assert(kABytes % 1024 == 0 && kBBytes % 1024 == 0, "swizzle-128B needs 1024 B aligned stages");
+
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint8_t* smem_cd = smem;
+    uint8_t* smem_a = smem + kCdBufs * kCdBufBytes;
+    uint8_t* smem_b = smem_a + kStages * kABytes;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + kStages * kBBytes);  // [kStages] TMA -> wgmma
+    uint64_t* empty_bar = full_bar + kStages;                                       // [kStages] wgmma -> TMA
+
+    const uint32_t warp_idx = threadIdx.x / 32;
+    const uint32_t lane = lane_id();
+    const uint32_t wg = warp_idx / 4;  // 0: producer + all-gather copier, 1-2: consumers
+    if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) {  // SWIZZLE_128B tiles must start on a 1024-byte boundary
+        printf("[b200] gemm: dynamic shared memory is not 1024-byte aligned\n");
+        __trap();
+    }
+
+    if (warp_idx == 0 && elect_one()) {
+        prefetch_tmap(&tmap_a);
+        prefetch_tmap(&tmap_b);
+        prefetch_tmap(&tmap_d);
+        if (p.epi.has_aux_out) prefetch_tmap(&tmap_aux);
+        for (int i = 0; i < kStages; ++i) {
+            mbar_init(&full_bar[i], 1);               // the producer's expect_tx arrive
+            mbar_init(&empty_bar[i], kConsumerWgs * 4);  // lane 0 of every consumer warp
+        }
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    const int tiles_per_batch = p.m_tiles * p.n_tiles;
+    const int total_tiles = tiles_per_batch * p.batch;
+    const int num_kb = (p.K + kBlockK - 1) / kBlockK;
+    const int kGroupN = p.group_n;  // n-tiles per raster group (keeps a wave's A/B footprint L2-resident)
+
+    // Static persistent schedule: CTA c computes tiles c, c + grid, c + 2 grid, ...  The tiles in flight are a
+    // contiguous window of the raster, so co-running CTAs share A / B panels in L2.
+    auto decode_tile = [&](int t, int& b, int& mt, int& nt) {
+        b = t / tiles_per_batch;
+        const int r = t - b * tiles_per_batch;
+        const int per_group = p.m_tiles * kGroupN;
+        const int g = r / per_group;
+        const int first_n = g * kGroupN;
+        const int gsz = min(kGroupN, p.n_tiles - first_n);
+        const int in_g = r - g * per_group;
+        mt = in_g / gsz;
+        nt = first_n + in_g % gsz;
+        nt += p.n_rot;  // AG fusion: start with the n-tiles of the locally owned slab
+        if (nt >= p.n_tiles) nt -= p.n_tiles;
+    };
+    const int ag_chunks_per_slab =
+        p.ag.world > 1 ? static_cast<int>((p.ag.slab_bytes + kAgChunkBytes - 1) / kAgChunkBytes) : 0;
+
+    if (wg == 0) {
+        reg_dealloc<56>();
+        if (warp_idx == 0) {
+            // ================================= TMA producer =================================
+            if (elect_one()) {
+                uint32_t stage = 0, phase = 0;
+                for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+                    int b, mt, nt;
+                    decode_tile(t, b, mt, nt);
+                    const int bi = b % p.nb_inner, bo = b / p.nb_inner;
+                    const int m_idx = mt * kBlockM;
+                    const int n_idx = nt * BLOCK_N;
+                    if (p.ag.world > 1) {
+                        // B rows [n_idx, n_idx + BLOCK_N) must have been pulled into the local gathered buffer
+                        const int last_row = min(n_idx + BLOCK_N, p.N) - 1;
+                        if (last_row >= n_idx) {
+                            const int s_lo = min(n_idx / p.ag.rows_per_slab, p.ag.world - 1);
+                            const int s_hi = min(last_row / p.ag.rows_per_slab, p.ag.world - 1);
+                            for (int sl = s_lo; sl <= s_hi; ++sl) {
+                                uint32_t spins = 0;
+                                while (ld_acquire_gpu(p.ag.flags + sl) < static_cast<uint32_t>(ag_chunks_per_slab)) {
+                                    if (++spins > (1u << 26)) {
+                                        printf("[b200] AG-fused GEMM: slab %d never arrived (block %d)\n", sl, blockIdx.x);
+                                        __trap();
+                                    }
+                                }
+                            }
+                            fence_proxy_async_all();  // generic-proxy peer copies -> async-proxy (TMA) reads
+                        }
+                    }
+                    for (int kb = 0; kb < num_kb; ++kb) {
+                        mbar_wait(&empty_bar[stage], phase ^ 1);
+                        const int k_idx = kb * kBlockK;
+                        uint8_t* sa = smem_a + stage * kABytes;
+                        uint8_t* sb = smem_b + stage * kBBytes;
+                        mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);  // out-of-bounds box parts count too
+                        if constexpr (kMajorA == 0) {
+                            tma_load_4d(&tmap_a, &full_bar[stage], sa, k_idx, m_idx, bi, bo);
+                        } else {
+#pragma unroll
+                            for (int i = 0; i < kBlockM / 64; ++i)
+                                tma_load_4d(&tmap_a, &full_bar[stage], sa + i * (64 * kBlockK * 2), m_idx + i * 64,
+                                                 k_idx, bi, bo);
+                        }
+                        if constexpr (kMajorB == 0) {
+                            tma_load_4d(&tmap_b, &full_bar[stage], sb, k_idx, n_idx, bi, bo);
+                        } else {
+#pragma unroll
+                            for (int i = 0; i < BLOCK_N / 64; ++i)
+                                tma_load_4d(&tmap_b, &full_bar[stage], sb + i * (64 * kBlockK * 2), n_idx + i * 64,
+                                                 k_idx, bi, bo);
+                        }
+                        stage = (stage + 1 == kStages) ? 0 : stage + 1;
+                        phase ^= (stage == 0);
+                    }
+                }
+            }
+        } else if (warp_idx == 1) {
+            // ================================= All-gather copier (AG fusion only) =================================
+            if (p.ag.world > 1) {
+                const int total_chunks = p.ag.world * ag_chunks_per_slab;
+                uint32_t* chunk_counter = p.ag.flags + p.ag.world;  // zeroed with the flags
+                for (;;) {
+                    int c = 0;
+                    if (lane == 0) c = static_cast<int>(atomicAdd(chunk_counter, 1u));
+                    c = __shfl_sync(0xffffffffu, c, 0);
+                    if (c >= total_chunks) break;
+                    const int k = c / ag_chunks_per_slab;            // arrival index: 0 = own slab
+                    const int sl = (p.ag.rank + k) % p.ag.world;      // slab pulled now (ranks start at different peers)
+                    const int64_t off = static_cast<int64_t>(c - k * ag_chunks_per_slab) * kAgChunkBytes;
+                    const int64_t nbytes = min(static_cast<int64_t>(kAgChunkBytes), p.ag.slab_bytes - off);
+                    const uint8_t* src = reinterpret_cast<const uint8_t*>(p.ag.peer_src[sl]) + off;
+                    uint8_t* dst = static_cast<uint8_t*>(p.ag.dst) + static_cast<int64_t>(sl) * p.ag.slab_bytes + off;
+                    const int nvec = static_cast<int>(nbytes / 16);
+                    int i = lane;
+                    for (; i + 3 * 32 < nvec; i += 4 * 32) {
+                        uint4 v[4];
+#pragma unroll
+                        for (int u = 0; u < 4; ++u) v[u] = ld_peer_v4(src + static_cast<int64_t>(i + u * 32) * 16);
+#pragma unroll
+                        for (int u = 0; u < 4; ++u) *reinterpret_cast<uint4*>(dst + static_cast<int64_t>(i + u * 32) * 16) = v[u];
+                    }
+                    for (; i < nvec; i += 32) *reinterpret_cast<uint4*>(dst + static_cast<int64_t>(i) * 16) = ld_peer_v4(src + static_cast<int64_t>(i) * 16);
+                    __threadfence();
+                    __syncwarp();
+                    if (lane == 0) red_release_gpu_add(p.ag.flags + sl, 1);
+                }
+            }
+        }
+    } else {
+        // ================================= Consumer warpgroups: wgmma + epilogue =================================
+        // Warpgroup w owns rows [64 w, 64 w + 64) of the 128 x BLOCK_N tile: one m64nNk16 wgmma per 16-wide k step,
+        // fp32 accumulators in registers.  One k-block of MMAs stays in flight while the next one is issued; the smem
+        // slot of a k-block is handed back to the producer as soon as its MMAs retired.
+        reg_alloc<224>();
+        const uint32_t cw = wg - 1;                       // consumer warpgroup index = 64-row slab of the tile
+        const uint32_t etid = threadIdx.x & 127;
+        const uint32_t wrow = (warp_idx & 3) * 16 + lane / 4;  // this thread's accumulator rows: wrow and wrow + 8
+        const uint32_t cpair = (lane & 3) * 2;            // first of its two adjacent columns inside every 8-column group
+        const uint32_t bar_id = 1 + cw;
+        uint8_t* const grp_buf = smem_cd + cw * 2 * kCdBufBytes;  // two 64 x 64 staging buffers per warpgroup
+        const GemmEpilogue& e = p.epi;
+        const bool ext_is_aux = e.act == kActDGelu;
+        // K-major : 8-row groups are 1024 B apart (SBO); one swizzle atom along K so LBO is unused.
+        // MN-major: 8-k groups are 1024 B apart (SBO); 64-wide MN atoms are BLOCK_K * 128 B apart (LBO).
+        constexpr uint32_t kLbo = kBlockK * 128;
+        constexpr uint32_t kKStepA = kMajorA == 0 ? (kMmaK * 2) : (kMmaK * 128);  // bytes per 16-wide k step
+        constexpr uint32_t kKStepB = kMajorB == 0 ? (kMmaK * 2) : (kMmaK * 128);
+        constexpr uint32_t kSlabA = 64 * kBlockK * 2;     // both majors: the warpgroup's 64 rows are 8 KB further
+        uint32_t stage = 0, phase = 0;
+        uint32_t flip = 0;
+        float d[BLOCK_N / 2];
+
+        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+            int b, mt, nt;
+            decode_tile(t, b, mt, nt);
+            const int bi = b % p.nb_inner, bo = b / p.nb_inner;
+            const int m0 = mt * kBlockM + cw * 64;
+            const int n0 = nt * BLOCK_N;
+
+            uint32_t prev_stage = 0;
+            for (int kb = 0; kb < num_kb; ++kb) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint32_t a_addr = smem_u32(smem_a + stage * kABytes) + cw * kSlabA;
+                const uint32_t b_addr = smem_u32(smem_b + stage * kBBytes);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kBlockK / kMmaK; ++k) {
+                    const uint64_t da = make_wgmma_desc(a_addr + k * kKStepA, kLbo, 1024, 1);
+                    const uint64_t db = make_wgmma_desc(b_addr + k * kKStepB, kLbo, 1024, 1);
+                    WgmmaSS<BLOCK_N, kMajorA, kMajorB>::mma(d, da, db, (kb > 0 || k > 0) ? 1u : 0u);
+                }
+                wgmma_commit();
+                if (kb > 0) {
+                    wgmma_wait<1>();  // the previous k-block's MMAs are done reading their slot
+                    if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+                }
+                prev_stage = stage;
+                stage = (stage + 1 == kStages) ? 0 : stage + 1;
+                phase ^= (stage == 0);
+            }
+            wgmma_wait<0>();
+            if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+            // ---- epilogue: registers -> swizzled staging buffer -> TMA store, 64 columns at a time ----
+            const int row0 = m0 + static_cast<int>(wrow), row1 = row0 + 8;
+            const bool row0_ok = row0 < p.M, row1_ok = row1 < p.M;
+            const __nv_bfloat16 *ext0 = nullptr, *ext1 = nullptr;
+            if (ext_is_aux) {
+                ext0 = e.aux_in + static_cast<int64_t>(row0) * e.ld_aux;
+                ext1 = e.aux_in + static_cast<int64_t>(row1) * e.ld_aux;
+            } else if (e.residual != nullptr) {
+                ext0 = e.residual + static_cast<int64_t>(e.res_row_mod > 0 ? row0 % e.res_row_mod : row0) * e.ld_res;
+                ext1 = e.residual + static_cast<int64_t>(e.res_row_mod > 0 ? row1 % e.res_row_mod : row1) * e.ld_res;
+            }
+#pragma unroll
+            for (int c = 0; c < BLOCK_N / 64; ++c) {
+                const int ncol0 = n0 + c * 64;
+                if (ncol0 >= p.N) continue;  // warpgroup-uniform: nothing to store
+                uint8_t* buf0 = grp_buf + (e.has_aux_out ? 0 : (flip & 1)) * kCdBufBytes;
+                uint8_t* buf1 = grp_buf + kCdBufBytes;
+                if (etid == 0) {  // staging buffer(s) of this warpgroup free again?
+                    if (e.has_aux_out)
+                        tma_store_wait_read<0>();
+                    else
+                        tma_store_wait_read<1>();
+                }
+                named_bar_sync(bar_id, kEpiThreads);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int col = ncol0 + j * 8 + static_cast<int>(cpair);
+                    const bool c0_ok = col < p.N, c1_ok = col + 1 < p.N;
+                    float v[4] = {d[(c * 8 + j) * 4], d[(c * 8 + j) * 4 + 1], d[(c * 8 + j) * 4 + 2], d[(c * 8 + j) * 4 + 3]};
+                    uint32_t x0 = 0, x1 = 0;  // dGELU pre-activation or residual of (row0 | row1, col..col+1)
+                    if (ext0 != nullptr && c0_ok) {
+                        if (row0_ok) x0 = __ldg(reinterpret_cast<const uint32_t*>(ext0 + col));
+                        if (row1_ok) x1 = __ldg(reinterpret_cast<const uint32_t*>(ext1 + col));
+                    }
+                    if (e.bias != nullptr && c0_ok) {
+                        const uint32_t bw = __ldg(reinterpret_cast<const uint32_t*>(e.bias + col));
+                        v[0] += bf16_lo(bw), v[1] += bf16_hi(bw), v[2] += bf16_lo(bw), v[3] += bf16_hi(bw);
+                    }
+                    // 16-byte chunk j of a 128-byte row, XOR-swizzled with the row like the TMA store expects
+                    const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
+                    const uint32_t off1 = off0 + 8 * 128;  // row + 8 has the same (row & 7)
+                    if (e.has_aux_out) {
+                        st_shared_b32(smem_u32(buf1) + off0, pack_bf16x2(v[0], v[1]));
+                        st_shared_b32(smem_u32(buf1) + off1, pack_bf16x2(v[2], v[3]));
+                    }
+                    if (e.act == kActGelu) {
+#pragma unroll
+                        for (int q = 0; q < 4; ++q) v[q] = gelu_erf(v[q]);
+                    } else if (ext_is_aux) {
+                        v[0] *= dgelu_erf(bf16_lo(x0)), v[1] *= dgelu_erf(bf16_hi(x0));
+                        v[2] *= dgelu_erf(bf16_lo(x1)), v[3] *= dgelu_erf(bf16_hi(x1));
+                    }
+                    if (e.residual != nullptr && !ext_is_aux) {
+                        v[0] += bf16_lo(x0), v[1] += bf16_hi(x0), v[2] += bf16_lo(x1), v[3] += bf16_hi(x1);
+                    }
+                    // rows / columns outside the problem are clipped by the TMA store; zeros keep the column sums clean
+                    if (!(row0_ok && c0_ok)) v[0] = 0.f;
+                    if (!(row0_ok && c1_ok)) v[1] = 0.f;
+                    if (!(row1_ok && c0_ok)) v[2] = 0.f;
+                    if (!(row1_ok && c1_ok)) v[3] = 0.f;
+                    st_shared_b32(smem_u32(buf0) + off0, pack_bf16x2(v[0], v[1]));
+                    st_shared_b32(smem_u32(buf0) + off1, pack_bf16x2(v[2], v[3]));
+                }
+                fence_proxy_async_smem();
+                named_bar_sync(bar_id, kEpiThreads);
+                if (etid == 0) {
+                    tma_store_4d(&tmap_d, buf0, ncol0, m0, bi, bo);
+                    tma_store_commit();
+                    if (e.has_aux_out) {
+                        tma_store_4d(&tmap_aux, buf1, ncol0, m0, bi, bo);
+                        tma_store_commit();
+                    }
+                }
+                if (e.colsum != nullptr) {
+                    // Bias gradient: column sums of the (bf16-rounded) output tile, fp32 atomics.
+                    const int ccol = etid & 63;       // column within the chunk
+                    const int rhalf = etid >> 6;      // 0/1 -> rows [0,32) / [32,64)
+                    const int jj = ccol >> 3, within = ccol & 7;
+                    float s = 0.f;
+#pragma unroll 8
+                    for (int r = 0; r < 32; ++r) {
+                        const int rr = rhalf * 32 + r;
+                        const uint8_t* ptr = buf0 + rr * 128 + ((jj ^ (rr & 7)) * 16) + within * 2;
+                        s += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(ptr));
+                    }
+                    if (ncol0 + ccol < p.N)
+                        atomicAdd(e.colsum + static_cast<int64_t>(bi) * e.colsum_bi_stride + ncol0 + ccol, s);
+                }
+                ++flip;
+            }
+        }
+        if (etid == 0) tma_store_wait<0>();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Host side
+// ------------------------------------------------------------------------------------------------
+using EncodeFn = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                              const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                              CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+EncodeFn get_encode_fn() {
+    static EncodeFn fn = nullptr;
+    static std::once_flag once;
+    std::call_once(once, [] {
+        void* sym = nullptr;
+        cudaDriverEntryPointQueryResult qres;
+        cudaError_t err = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &sym, cudaEnableDefault, &qres);
+        if (err != cudaSuccess || qres != cudaDriverEntryPointSuccess || sym == nullptr)
+            throw std::runtime_error("cuTensorMapEncodeTiled not available from the driver");
+        fn = reinterpret_cast<EncodeFn>(sym);
+    });
+    return fn;
+}
+
+struct TmapKey {
+    uint64_t ptr;
+    int64_t d[4];
+    int64_t s[3];
+    int32_t box[2];
+    bool operator==(const TmapKey& o) const { return std::memcmp(this, &o, sizeof(TmapKey)) == 0; }
+};
+struct TmapKeyHash {
+    size_t operator()(const TmapKey& k) const {
+        const uint64_t* w = reinterpret_cast<const uint64_t*>(&k);
+        size_t h = 1469598103934665603ull;
+        for (size_t i = 0; i < sizeof(TmapKey) / 8; ++i) h = (h ^ w[i]) * 1099511628211ull;
+        return h;
+    }
+};
+
+// 4-D bf16 tensor map: dims (inner, outer, batch_inner, batch_outer), box (box_inner, box_outer, 1, 1).
+CUtensorMap make_tmap(const GemmOperand& op, int64_t inner, int64_t outer, int box_inner, int box_outer,
+                      int swizzle_bytes = 128) {
+    static std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> cache;
+    static std::mutex mu;
+    TmapKey key;
+    std::memset(&key, 0, sizeof(key));
+    key.ptr = reinterpret_cast<uint64_t>(op.ptr);
+    key.d[0] = inner, key.d[1] = outer, key.d[2] = op.nb_inner, key.d[3] = op.nb_outer;
+    key.s[0] = op.ld, key.s[1] = op.stride_b_inner, key.s[2] = op.stride_b_outer;
+    key.box[0] = box_inner, key.box[1] = box_outer + (swizzle_bytes << 16);
+    {
+        std::lock_guard<std::mutex> lock(mu);
+        auto it = cache.find(key);
+        if (it != cache.end()) return it->second;
+    }
+    if ((reinterpret_cast<uint64_t>(op.ptr) & 15) != 0) throw std::runtime_error("gemm: operand base must be 16 B aligned");
+    if ((op.ld * 2) % 16 != 0) throw std::runtime_error("gemm: leading dimension must be a multiple of 8 elements");
+    CUtensorMap tm;
+    cuuint64_t dims[4] = {static_cast<cuuint64_t>(inner), static_cast<cuuint64_t>(outer),
+                          static_cast<cuuint64_t>(op.nb_inner), static_cast<cuuint64_t>(op.nb_outer)};
+    // Strides of size-1 batch dims are irrelevant but must still be legal multiples of 16 B.
+    const int64_t sbi = op.nb_inner > 1 ? op.stride_b_inner : op.ld * outer;
+    const int64_t sbo = op.nb_outer > 1 ? op.stride_b_outer : sbi * op.nb_inner;
+    if ((sbi * 2) % 16 != 0 || (sbo * 2) % 16 != 0) throw std::runtime_error("gemm: batch strides must be multiples of 8 elements");
+    cuuint64_t strides[3] = {static_cast<cuuint64_t>(op.ld * 2), static_cast<cuuint64_t>(sbi * 2),
+                             static_cast<cuuint64_t>(sbo * 2)};
+    cuuint32_t box[4] = {static_cast<cuuint32_t>(box_inner), static_cast<cuuint32_t>(box_outer), 1, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult res = get_encode_fn()(&tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(op.ptr), dims, strides,
+                                   box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                                   swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                   : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                                         : CU_TENSOR_MAP_SWIZZLE_32B,
+                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (res != CUDA_SUCCESS) {
+        char msg[256];
+        snprintf(msg, sizeof(msg),
+                 "cuTensorMapEncodeTiled failed (%d): dims=(%lld,%lld,%lld,%lld) ld=%lld box=(%d,%d)", (int)res,
+                 (long long)inner, (long long)outer, (long long)op.nb_inner, (long long)op.nb_outer, (long long)op.ld,
+                 box_inner, box_outer);
+        throw std::runtime_error(msg);
+    }
+    std::lock_guard<std::mutex> lock(mu);
+    if (cache.size() > 4096) cache.clear();
+    cache.emplace(key, tm);
+    return tm;
+}
+
+int num_sms() {
+    static int n = 0;
+    if (n == 0) {
+        int dev = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    }
+    return n;
+}
+
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages>
+void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, const GemmOperand* aux, int M, int N,
+            int K, const GemmEpilogue& epi, int max_ctas, cudaStream_t stream, const GemmAgFuse* ag) {
+    constexpr int kSmem = kCdBufs * kCdBufBytes + kStages * (kBlockM + BLOCK_N) * kBlockK * 2 + 2 * kStages * 8;
+    static_assert(kSmem <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
+    auto kern = gemm_bf16_sm90_kernel<kMajorA, kMajorB, BLOCK_N, kStages>;
+    static bool attr_set = false;
+    if (!attr_set) {
+        cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+        if (err != cudaSuccess) throw std::runtime_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(err));
+        attr_set = true;
+    }
+    // A: K-major -> (inner=K, outer=M), box (64, 128).  MN-major -> (inner=M, outer=K), box (64, 64).
+    CUtensorMap ta = kMajorA == 0 ? make_tmap(A, K, M, kBlockK, kBlockM) : make_tmap(A, M, K, 64, kBlockK);
+    CUtensorMap tb = kMajorB == 0 ? make_tmap(B, K, N, kBlockK, BLOCK_N) : make_tmap(B, N, K, 64, kBlockK);
+    CUtensorMap td = make_tmap(D, N, M, 64, 64);
+    CUtensorMap tx = (epi.has_aux_out && aux != nullptr) ? make_tmap(*aux, N, M, 64, 64) : td;
+
+    KernelParams p;
+    p.M = M, p.N = N, p.K = K;
+    p.batch = static_cast<int>(D.nb_inner * D.nb_outer);
+    p.nb_inner = static_cast<int>(D.nb_inner);
+    p.m_tiles = (M + kBlockM - 1) / kBlockM;
+    p.n_tiles = (N + BLOCK_N - 1) / BLOCK_N;
+    p.epi = epi;
+    p.n_rot = 0;
+    // n-tiles per raster group: 2048 output columns.  Reasoning, not a measurement: a wave of 132 CTAs then covers
+    // ~16 m-tiles x 2048 columns, about as many A rows (2112) as B rows (2048), the split that fetches the fewest
+    // operand bytes per wave, and at K = 5120 both panels together (~43 MB) are below the 50 MB of L2.
+    p.group_n = 2048 / BLOCK_N;
+    if (ag != nullptr && ag->world > 1) {
+        if (kMajorB != 0 || p.batch != 1) throw std::runtime_error("gemm: AG fusion needs a K-major, un-batched B");
+        if (static_cast<int64_t>(ag->rows_per_slab) * K * 2 != ag->slab_bytes || ag->slab_bytes % 16 != 0)
+            throw std::runtime_error("gemm: AG fusion needs whole rows per slab");
+        p.ag = *ag;
+        p.n_rot = static_cast<int>((static_cast<int64_t>(ag->rank) * ag->rows_per_slab) / BLOCK_N) % p.n_tiles;
+        cudaMemsetAsync(ag->flags, 0, sizeof(uint32_t) * (ag->world + 1), stream);  // slab counters + chunk counter
+    }
+    const int64_t total = static_cast<int64_t>(p.m_tiles) * p.n_tiles * p.batch;
+    int sms = num_sms();
+    if (max_ctas > 0 && max_ctas < sms) sms = max_ctas;
+    const int ctas = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(total, sms)));
+    kern<<<ctas, kNumThreads, kSmem, stream>>>(ta, tb, td, tx, p);
+    cudaError_t err = cudaGetLastError();
+    if (err != cudaSuccess) throw std::runtime_error(std::string("gemm launch failed: ") + cudaGetErrorString(err));
+}
+
+}  // namespace
+
+CUtensorMap make_tensor_map_4d(const GemmOperand& op, int64_t inner, int64_t outer, int box_inner, int box_outer,
+                               int swizzle_bytes) {
+    return make_tmap(op, inner, outer, box_inner, box_outer, swizzle_bytes);
+}
+
+void gemm_bf16(const GemmOperand& A, int major_a, const GemmOperand& B, int major_b, const GemmOperand& D,
+               const GemmOperand* aux_out, int M, int N, int K, const GemmEpilogue& epi, int block_n, int max_ctas,
+               cudaStream_t stream, const GemmAgFuse* ag) {
+    if (N % 8 != 0 && (epi.residual || epi.aux_in))
+        throw std::runtime_error("gemm: N must be a multiple of 8 when residual/aux_in are used");
+    if (epi.act == kActDGelu && (epi.residual != nullptr || epi.aux_in == nullptr))
+        throw std::runtime_error("gemm: dGELU epilogue needs aux_in and cannot be combined with a residual");
+    if (D.nb_inner * D.nb_outer > 1 && (epi.bias || epi.residual || epi.aux_in))
+        throw std::runtime_error("gemm: bias/residual/aux_in are not supported for batched problems");
+    if (block_n == 0) block_n = (N > 128) ? 256 : 128;
+#define B200_DISPATCH(MA, MB, BN, ST)                                                             \
+    if (major_a == MA && major_b == MB && block_n == BN) {                                        \
+        launch<MA, MB, BN, ST>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);             \
+        return;                                                                                   \
+    }
+    B200_DISPATCH(0, 0, 256, 4)
+    B200_DISPATCH(0, 1, 256, 4)
+    B200_DISPATCH(1, 1, 256, 4)
+    B200_DISPATCH(1, 0, 256, 4)
+    B200_DISPATCH(0, 0, 128, 6)
+    B200_DISPATCH(0, 1, 128, 6)
+    B200_DISPATCH(1, 1, 128, 6)
+    B200_DISPATCH(1, 0, 128, 6)
+#undef B200_DISPATCH
+    throw std::runtime_error("gemm: unsupported (major_a, major_b, block_n) combination");
+}
+
+}  // namespace b200

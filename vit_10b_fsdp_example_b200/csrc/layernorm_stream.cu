@@ -1,10 +1,8 @@
 // LayerNorm backward for wide rows (D >= 2048) as a bulk-copy pipeline.
 //
-// The register-resident kernel in elementwise.cu is *issue*-bound, not memory-bound, inside a training step: ncu at
-// boost clocks reads 0.41 ms (51 % of HBM), but under the 1 kW power cap the SMs run at ~1.3 GHz next to the GEMMs and
-// the same kernel takes 0.63 ms (CUPTI trace, profiles/r2_timeline.md) -- its per-row shared-memory read-modify-write of
-// 3 x D column accumulators, two block barriers per row and a half-empty third chunk (D = 5120 over 256 threads) cost
-// more instructions than the 1.34 GB of traffic costs time.  This version:
+// The register-resident kernel in elementwise.cu pays, per row, a shared-memory read-modify-write of 3 x D column
+// accumulators, two block barriers and a half-empty third chunk (D = 5120 over 256 threads): many instructions per
+// byte moved.  (Neither kernel has been timed on H100.)  This version:
 //   * one producer thread streams whole rows (x, dy, residual gradient: one cp.async.bulk each, 10 KB at D = 5120)
 //     into a shared-memory ring of kStages rows, completion on mbarriers -- 90+ KB in flight per SM with zero
 //     register cost, so a single CTA per SM saturates HBM;
@@ -182,7 +180,7 @@ __global__ void __launch_bounds__(kMaxThreads, 1)
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[st]);  // this warp no longer reads the stage
     }
-    // one global atomic per column per CTA (148 arrivals per address)
+    // one global atomic per column per CTA (one arrival per SM per address)
 #pragma unroll
     for (int v = 0; v < kVPT; ++v) {
         const int c0 = (ct + v * ncons) * 8;

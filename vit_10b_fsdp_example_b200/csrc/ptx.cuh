@@ -1,6 +1,6 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) execution model:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM alloc / ld / commit / fence),
-// cluster helpers and NVLink multimem instructions.
+// Thin inline-PTX wrappers for the Hopper (sm_90a) execution model:
+// mbarrier, TMA (cp.async.bulk.tensor), cluster helpers, register reallocation and small packing helpers.
+// The wgmma wrappers live in wgmma.cuh.
 //
 // Everything here is hand-written PTX; no CUTLASS/CuTe dependency.
 #pragma once
@@ -12,7 +12,7 @@
 namespace b200 {
 
 #ifndef B200_SPIN_LIMIT
-// Bounded spin: a stuck barrier traps (-> launch error) instead of hanging the GPU box.
+// Bounded spin: a stuck barrier traps (-> launch error) instead of hanging the GPU.
 // ~2^31 polls of a try_wait with a HW suspend-time hint is many seconds.
 #define B200_SPIN_LIMIT (1u << 28)
 #endif
@@ -134,32 +134,6 @@ __device__ __forceinline__ void tma_load_4d(const void* tmap, uint64_t* bar, voi
         : "memory");
 }
 
-// 4-D tiled load, 2-CTA flavour: data lands in *this* CTA's smem, the transaction bytes are
-// credited to the barrier at the same offset in the even (leader) CTA of the pair.
-__device__ __forceinline__ void tma_load_4d_2cta(const void* tmap, uint64_t* bar, void* smem, int c0, int c1,
-                                                 int c2, int c3) {
-    const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(smem)),
-        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_leader), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-
-// Same, with an L2 eviction-priority hint (createpolicy-encoded 64-bit immediate).
-constexpr uint64_t kL2EvictNormal = 0x1000000000000000ull;
-constexpr uint64_t kL2EvictFirst = 0x12F0000000000000ull;
-constexpr uint64_t kL2EvictLast = 0x14F0000000000000ull;
-__device__ __forceinline__ void tma_load_4d_2cta_hint(const void* tmap, uint64_t* bar, void* smem, int c0, int c1,
-                                                      int c2, int c3, uint64_t policy) {
-    const uint32_t bar_leader = smem_u32(bar) & 0xFEFFFFFFu;
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-        " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(smem)),
-        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar_leader), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(policy)
-        : "memory");
-}
-
 __device__ __forceinline__ void tma_store_4d(const void* tmap, const void* smem, int c0, int c1, int c2, int c3) {
     asm volatile(
         "cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"(
@@ -180,130 +154,15 @@ __device__ __forceinline__ void tma_store_wait() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// Register reallocation between the producer and the consumer warpgroups
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                     "r"(ncols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    } else {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                     "r"(ncols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
+template <int N>
+__device__ __forceinline__ void reg_dealloc() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
-
-template <int kCtaGroup>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-    } else {
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-    }
-}
-
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs / fp32 accumulate.
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-            "}\n" ::"r"(tmem_d),
-            "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-            : "memory");
-    } else {
-        asm volatile(
-            "{\n\t"
-            ".reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-            "}\n" ::"r"(tmem_d),
-            "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-            : "memory");
-    }
-}
-
-// Make `bar` track completion of all previously issued tcgen05.mma of this thread.
-// (implies tcgen05.fence::before_thread_sync)
-template <int kCtaGroup>
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    if constexpr (kCtaGroup == 1) {
-        asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                         smem_u32(bar))
-                     : "memory");
-    } else {
-        const uint16_t mask = 3;
-        asm volatile(
-            "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-                "r"(smem_u32(bar)),
-            "h"(mask)
-            : "memory");
-    }
-}
-
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp receives row (lane_base + t).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------------------------
-// Descriptors
-// ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (sm_100 "version 1"), SWIZZLE_128B.
-//   bits [ 0,14) start address >> 4      bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4 bits [46,48) version = 1
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
-    return d;
-}
-
-// Generic form of the descriptor above: layout 2 = SWIZZLE_128B, 4 = SWIZZLE_64B.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint32_t layout) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(layout) << 61;
-    return d;
-}
-
-// Instruction descriptor for kind::f16 with bf16 A/B and fp32 D.
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt (1 = bf16)  [10,13) B fmt (1 = bf16)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t m, uint32_t n, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((n >> 3) << 17) |
-           ((m >> 4) << 24);
+template <int N>
+__device__ __forceinline__ void reg_alloc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -318,6 +177,10 @@ __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v 
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t a) {
+    asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
 }
 
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {

@@ -56,7 +56,7 @@ class FakeBatchLoader:
 
 class DevicePrefetcher:
     """Iterates a host loader and keeps ``depth`` batches in flight on a dedicated copy stream
-    (pinned memory + non_blocking copies), the B200 analogue of ``pl.MpDeviceLoader``."""
+    (pinned memory + non_blocking copies), the CUDA analogue of ``pl.MpDeviceLoader``."""
 
     def __init__(self, loader, device: torch.device, depth: int = 2):
         self.loader, self.device, self.depth = loader, device, max(1, depth)

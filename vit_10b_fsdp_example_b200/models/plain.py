@@ -1,7 +1,7 @@
 """A plain (un-sharded, autograd) ``nn.Module`` ViT with timm-compatible parameter names.
 
 This is the consumer side of the checkpoint contract: the reference's per-rank files exist so that an offline tool
-can rebuild a full ``state_dict`` "loadable into a plain (non-FSDP) ViT" (utils.py:27-28, SURVEY 5.4).
+can rebuild a full ``state_dict`` "loadable into a plain (non-FSDP) ViT" (utils.py:27-28).
 ``PlainViT.load_state_dict(consolidated, strict=True)`` accepts exactly what ``consolidate_sharded_ckpts`` writes.
 The architecture is the reference's FSDPViTModel (run_vit_training.py:99-162) without the wrappers: conv patch embed,
 learned position embedding, pre-LN blocks (LayerNorm eps 1e-5), final LayerNorm (eps 1e-6), mean pool, linear head.

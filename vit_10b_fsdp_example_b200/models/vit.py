@@ -10,7 +10,7 @@ Parameter names are timm-compatible (``norm1.weight``, ``attn.qkv.weight``, ``ml
 There is no autograd here: every stage has an explicit backward, which is what lets the FSDP engine
 place every gather / reduce-scatter / free deterministically and write weight gradients straight into
 the flat per-unit gradient buffer.  ``ops`` is either ``torch_ops`` (reference, CPU) or ``cuda_ops``
-(sm_100a kernels); both expose the same functions.
+(sm_90a kernels); both expose the same functions.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Functional op sets: ``torch_ops`` (reference / CPU) and ``cuda_ops`` (hand-written sm_100a kernels)."""
+"""Functional op sets: ``torch_ops`` (reference / CPU) and ``cuda_ops`` (hand-written sm_90a kernels)."""
 from . import torch_ops  # noqa: F401
 
 

@@ -1,12 +1,12 @@
-"""sm_100a implementation of the functional op set (same contract as ``torch_ops``).
+"""sm_90a implementation of the functional op set (same contract as ``torch_ops``).
 
 Every function launches hand-written kernels from ``_C.so``:
-  * GEMMs: persistent 2-CTA tcgen05 kernel with TMEM accumulators and fused epilogues
+  * GEMMs: persistent warp-specialised wgmma kernel (TMA ring, register accumulators) with fused epilogues
     (bias / GELU / dGELU / residual / pre-activation side output / bias-gradient column sums);
     forward (NT), dgrad (NN) and wgrad (TN) run on the same kernel via K-major / MN-major descriptors.
-  * attention core: fused tcgen05 forward (keeps the row log-sum-exp) + fused backward kernels that read q/k/v in
+  * attention core: fused wgmma forward (keeps the row log-sum-exp) + fused backward kernels that read q/k/v in
     place from the packed qkv buffer through 4-D TMA tensor maps; scores never reach HBM.  The un-fused path (batched
-    tcgen05 GEMMs + softmax / softmax-backward kernels with materialised P) remains for attention dropout and
+    wgmma GEMMs + softmax / softmax-backward kernels with materialised P) remains for attention dropout and
     B200_FUSED_ATTN_BWD=0.
   * LayerNorm fwd/bwd, cross-entropy, im2col, column sums, sum of squares, fused AdamW.
 
@@ -61,7 +61,8 @@ def launch_count() -> int:
 
 ACT_NONE, ACT_GELU, ACT_DGELU = 0, 1, 2
 # GELU / dGELU are fused into the GEMM epilogue only when the reduction is deep enough to hide the math
-# (ViT-10B: K = 5120 fused; ViT-L: K = 1024 -> plain GEMM + stand-alone elementwise kernel, measured 1.5x faster)
+# (ViT-10B: K = 5120 fused; ViT-L: K = 1024 -> plain GEMM + stand-alone elementwise kernel; the threshold has not
+# been re-measured on H100)
 import os as _os
 
 FUSE_ACT_MIN_K = int(_os.environ.get("B200_FUSE_ACT_MIN_K", "2048"))
@@ -212,18 +213,6 @@ def colsum(x):
 # Attention core
 # ------------------------------------------------------------------------------------------------
 FUSED_ATTENTION = _os.environ.get("B200_FUSED_ATTN", "1") != "0"
-FUSED_ATTENTION_HD160 = _os.environ.get("B200_FUSED_ATTN_HD160", "0") == "1"
-
-
-# Persistent, software-pipelined kernels (csrc/attention_persist_sm100.cu, attention_bwd_persist_sm100.cu): one CTA per
-# SM loops over work items.  They win where only one CTA fits an SM (hd = 160, round-2 kernels: forward 311 vs 763 us
-# one-shot, backward 1352 vs 1814 us) and lose where two fit (hd = 64: 254 vs 159 us), hence the per-shape default below.
-_PERSIST_ENV = _os.environ.get("B200_ATTN_PERSIST", "")
-ATTN_PERSIST = _PERSIST_ENV == "1"
-
-
-def _persist(hd: int) -> bool:
-    return ATTN_PERSIST or (_PERSIST_ENV != "0" and hd > 128)
 
 
 def dropout(x, p: float, key: int):
@@ -262,15 +251,9 @@ def attention_fwd(qkv, B: int, N: int, H: int, hd: int, drop=None, need_p: bool 
         gemm_raw(pd, ldp, 0, qkv[:, 2 * D:], ld3, 1, out, D, N, hd, N,
                  batch=(H, B, N * ldp, H * N * ldp, hd, N * ld3, hd, N * D))
         return out, p
-    if _persist(hd) and FUSED_ATTENTION and not need_p and _C.attention_fwd_persist_supported(N, hd):
-        out = torch.empty(B * N, D, dtype=qkv.dtype, device=qkv.device)
-        _C.attention_fwd_persist(qkv, out, None, B, N, H, hd)
-        return out, None
-    # hd <= 128: two CTAs fit an SM and the one-shot fused kernel is ~1.8x faster than GEMM+softmax+GEMM (ViT-L: 159 vs
-    # 279 us).  hd = 160 (ViT-10B) needs 200 KB of smem -> one CTA per SM: that shape runs the persistent kernel above
-    # (311 us); the one-shot kernel (764 us) loses to the batched-GEMM path (664 us) there and is only used when forced.
-    if FUSED_ATTENTION and _C.attention_fwd_supported(N, hd) and (hd <= 128 or FUSED_ATTENTION_HD160):
-        # one fused tcgen05 kernel per (image, head, 128-query block): S and P live in TMEM / shared memory
+    # Fused kernel (S and P live in registers).  With P requested it is still faster than GEMM + softmax + GEMM:
+    # 1445 vs 1996 us at B128 N256 H32 hd160, 383 vs 654 us at B128 N196 H16 hd64 (CUDA events, H100 80GB HBM3, 700 W).
+    if FUSED_ATTENTION and _C.attention_supported(N, hd):
         out = torch.empty(B * N, D, dtype=qkv.dtype, device=qkv.device)
         p = None
         if need_p:
@@ -296,54 +279,33 @@ def attention_fwd(qkv, B: int, N: int, H: int, hd: int, drop=None, need_p: bool 
 
 
 # Fused (flash-style) forward + backward pair: the forward keeps only the row log-sum-exp, the backward kernels
-# (csrc/attention_bwd_sm100.cu) rebuild P tile by tile; scores never reach HBM.  Measured on B200 (CUDA events,
-# profiles/r2_attention.md), forward + backward incl. the P re-materialisation the un-fused path needs:
-#   ViT-L  (B128 N196 H16 hd64) : fused 159 + 387 us   vs un-fused 279 + 500 + 204 us   -> fused by default
-#   336 px (B56 N576 H32 hd160) : fused 1584 + 3032 us vs un-fused 1424 + 2459 + 1088 us, and P alone would be
-#                                 1.2 GB per block                                       -> fused by default
-#   ViT-10B (B128 N256 H32 hd160): fused (persistent, round 2) 311 + 1352 us vs un-fused 664 + 1356 (+426 if P is not
-#                                 kept), and no 512 MiB of P per block                   -> fused by default
-# B200_FUSED_ATTN_BWD=0 / 1 forces the choice.
-_FLASH_ENV = _os.environ.get("B200_FUSED_ATTN_BWD", "")
-FLASH_ATTENTION = _FLASH_ENV != "0"
-FLASH_LONG = _os.environ.get("B200_FUSED_ATTN_LONG", "1") != "0"
+# (csrc/attention_sm90.cu) rebuild P tile by tile; scores never reach HBM and no [B*H, N, N] buffer is allocated (at
+# the ViT-10B shape P alone would be 512 MiB per block).  Fused by default; B200_FUSED_ATTN_BWD=0 selects the un-fused path.
+FLASH_ATTENTION = _os.environ.get("B200_FUSED_ATTN_BWD", "") != "0"
 
 
 def flash_supported(N: int, hd: int) -> bool:
-    if N <= 256:
-        return bool(_C.attention_fwd_supported(N, hd) and _C.attention_bwd_supported(N, hd))
-    return bool(FLASH_LONG and _C.attention_fwd_long_supported(N, hd) and _C.attention_bwd_supported(N, hd))
+    return bool(_C.attention_supported(N, hd))
 
 
 def use_flash(N: int, hd: int) -> bool:
     """Model-level policy: run the attention core through the fused forward (log-sum-exp) + fused backward pair?"""
-    if not FLASH_ATTENTION or not flash_supported(N, hd):
-        return False
-    return True
+    return FLASH_ATTENTION and flash_supported(N, hd)
 
 
 def attention_fwd_lse(qkv, B: int, N: int, H: int, hd: int):
     out = torch.empty(B * N, H * hd, dtype=qkv.dtype, device=qkv.device)
     lse = torch.empty(B * H, N, dtype=torch.float32, device=qkv.device)
-    if _persist(hd) and _C.attention_fwd_persist_supported(N, hd):
-        _C.attention_fwd_persist(qkv, out, lse, B, N, H, hd)
-    elif N <= 256:
-        _C.attention_fwd(qkv, out, lse, None, B, N, H, hd)
-    else:
-        _C.attention_fwd_long(qkv, out, lse, B, N, H, hd)
+    _C.attention_fwd(qkv, out, lse, None, B, N, H, hd)
     return out, lse
 
 
 def attention_bwd_lse(dout, qkv, out, lse, B: int, N: int, H: int, hd: int, want_colsum: bool = False):
     dqkv = torch.empty(B * N, 3 * H * hd, dtype=qkv.dtype, device=qkv.device)
-    persist = _persist(hd) and N % 4 == 0  # the persistent kernels bulk-copy per-row statistics in 16-byte units
-    # scratch: rowsum(dO o O); the persistent kernels get a second plane holding lse * log2(e)
-    delta = torch.empty(2 if persist else 1, B * H, N, dtype=torch.float32, device=qkv.device)
-    # the persistent kernels reduce the qkv bias gradient (column sums of dq | dk | dv) from their epilogue tiles
-    cs = torch.zeros(3 * H * hd, dtype=torch.float32, device=qkv.device) if (want_colsum and persist) else None
-    _C.attention_bwd(qkv, dout, out, lse, delta, dqkv, cs, B, N, H, hd, persist)
-    if want_colsum and cs is None:
-        cs = colsum(dqkv)
+    delta = torch.empty(B * H, N, dtype=torch.float32, device=qkv.device)  # scratch: rowsum(dO o O)
+    # the backward kernels reduce the qkv bias gradient (column sums of dq | dk | dv) from their epilogue tiles
+    cs = torch.zeros(3 * H * hd, dtype=torch.float32, device=qkv.device) if want_colsum else None
+    _C.attention_bwd(qkv, dout, out, lse, delta, dqkv, cs, B, N, H, hd)
     return (dqkv, cs) if want_colsum else dqkv
 
 

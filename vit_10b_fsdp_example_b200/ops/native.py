@@ -1,6 +1,6 @@
 """Loader for the in-tree native extension (``vit_10b_fsdp_example_b200/_C.so``).
 
-The extension holds every hand-written sm_100a kernel.  It is built in-tree by
+The extension holds every hand-written sm_90a kernel.  It is built in-tree by
 ``vit_10b_fsdp_example_b200.build_ext`` so the ``.so`` travels with the repo snapshot.  On a machine
 with a GPU a missing extension is a hard error (no silent PyTorch fallback on the CUDA path).
 """

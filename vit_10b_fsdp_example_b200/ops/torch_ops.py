@@ -1,6 +1,6 @@
 """Reference implementation of the functional op set in plain PyTorch.
 
-This is (a) the CPU / gloo test backend, (b) the fp32 numerical oracle every sm_100a kernel is tested
+This is (a) the CPU / gloo test backend, (b) the fp32 numerical oracle every sm_90a kernel is tested
 against, and (c) the semantics contract for ``cuda_ops``.  Every function here has a same-named,
 same-signature twin in ``cuda_ops`` that runs the hand-written kernels.
 
@@ -154,7 +154,7 @@ def attention_fwd(qkv, B: int, N: int, H: int, hd: int, drop=None, need_p: bool 
 
 
 # Flash-style pair: the forward keeps only the log-sum-exp of every score row, the backward rebuilds P from it
-# (csrc/attention_bwd_sm100.cu on the GPU).  Off by default; tests flip FLASH_ATTENTION to exercise the model path.
+# (csrc/attention_sm90.cu on the GPU).  Off by default; tests flip FLASH_ATTENTION to exercise the model path.
 FLASH_ATTENTION = False
 
 

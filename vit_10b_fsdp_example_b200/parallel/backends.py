@@ -1,8 +1,8 @@
 """Collective backends of the FSDP engine.
 
 ``TorchDistBackend``  torch.distributed collectives (gloo on CPU, NCCL on GPU).  It is the CPU test vehicle
-                      and the honest NCCL baseline -- *not* the product path on B200.
-``Sm100Backend``      hand-written NVLink 5 / NVSwitch kernels over symmetric memory (csrc/comm.cu):
+                      and the honest NCCL baseline -- *not* the product path on H100.
+``Sm100Backend``      hand-written NVLink / NVSwitch kernels over symmetric memory (csrc/comm.cu):
                       sync-free peer-to-peer all-gather that lands shards in their final position,
                       one-pass reduce-scatter (+1/W mean, +fp32 cast, +grad-norm partial) with optional
                       in-switch NVLS reduction, flag barriers and scalar all-reduce.  No NCCL on the hot path.
@@ -128,12 +128,12 @@ class Sm100Backend(TorchDistBackend):
         from ..ops import native
 
         self._C = native.load()
-        # Collective kernels are light CTAs (128 threads, <= 96 registers, no shared memory) that run NEXT TO the
-        # GEMM CTAs on the same SMs (see csrc/comm.cu); comm_ctas bounds how many SMs host one at a time.
+        # Collective kernels are light CTAs (128 threads, <= 96 registers, no shared memory, see csrc/comm.cu);
+        # comm_ctas bounds how many of them one collective launches.  The value has not been tuned on H100.
         self.comm_ctas = int(os.environ.get("B200_COMM_CTAS", comm_ctas))
         # stand-alone all-gather transport: "kernel" = light pull kernel (csrc/comm.cu), "ce" = copy engines.
-        # SM-issued peer loads stop scaling beyond two GPUs on this fabric (305 GB/s at W = 2, 63 GB/s at W = 4) while
-        # DMA peer copies run at 636 GB/s and take nothing from the SMs, so the copy engines are the default.
+        # The copy engines take nothing from the SMs, so they are the default; the two transports have not been
+        # compared on H100.
         self.ag_transport = os.environ.get("B200_AG_TRANSPORT", "ce")
         self.use_nvls = False
         if world == 1:  # single GPU: nothing to communicate, gathered buffers alias the shards
@@ -211,8 +211,8 @@ class Sm100Backend(TorchDistBackend):
     def _ag_table(self, layout: UnitLayout, esize: int, exclude=()):
         """Segment table of the pull all-gather.  The order of the rows is the order in which this rank's CTAs walk
         the sources, so it is staggered by rank and rotated every MiB: at any moment the W ranks pull from W
-        *different* peers.  (With every rank walking the sources 0, 1, 2 ... in the same order all of them hit one
-        GPU's egress at once: measured 59 GB/s at W = 4 against 305 GB/s at W = 2, profiles/r2_n4.md.)"""
+        *different* peers.  (With every rank walking the sources 0, 1, 2 ... in the same order all of them would hit
+        one GPU's egress at once.)"""
         key = ("ag", self._lay_key(layout), esize, tuple(sorted(exclude)))
         if key not in self._seg_cache:
             chunk = self._C.ag_chunk_bytes()

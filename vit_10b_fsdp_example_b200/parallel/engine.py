@@ -47,7 +47,7 @@ class _NullEvent:
         pass
 
 
-# debug aid (SURVEY 5.2): overwrite a gathered-parameter buffer with NaN the moment the engine releases it, so any
+# debug aid: overwrite a gathered-parameter buffer with NaN the moment the engine releases it, so any
 # use-after-release of resharded parameters shows up as a NaN loss instead of silently reading stale weights
 DEBUG_POISON = os.environ.get("B200_DEBUG_POISON", "0") == "1"
 # NVTX ranges around every block's forward / backward (visible in nsys / ncu timelines)
@@ -113,7 +113,7 @@ class FSDPViT:
         if self.is_cuda:
             from ..ops import cuda_ops
 
-            assert dtype == torch.bfloat16, "the sm_100a kernel path is bf16 (use --device cpu for fp32 reference runs)"
+            assert dtype == torch.bfloat16, "the sm_90a kernel path is bf16 (use --device cpu for fp32 reference runs)"
             self.ops = cuda_ops
         else:
             from ..ops import torch_ops
@@ -128,9 +128,9 @@ class FSDPViT:
         self.step_count = 0        # optimizer steps since the start of training (checkpointed: seeds the dropout masks)
         self._steps_here = 0       # forward_backward calls of THIS process (the keep policy is sized after the first one)
         # All-gather fused into the qkv / fc1 GEMMs (copier warp pulling peer slabs with SM-issued loads): on by default
-        # at W = 2, where peer loads stream at ~300 GB/s; beyond two GPUs SM-issued peer loads drop to ~60 GB/s on this
-        # fabric (profiles/r2_n4.md) and the GEMM would wait for its weights, so the whole block is gathered by the
-        # copy engines instead.  B200_FUSE_AG=1 / 0 forces either way.
+        # at W = 2 only; with more peers one warp per CTA has to pull (W - 1) / W of the weight while the GEMM waits
+        # for it, so the whole block is gathered by the copy engines instead.  The crossover has not been measured on
+        # H100 (no multi-GPU run yet).  B200_FUSE_AG=1 / 0 forces either way.
         fuse_env = os.environ.get("B200_FUSE_AG", "")
         self.fuse_all_gather = fuse_all_gather and fuse_env != "0" and (world <= 2 or fuse_env == "1")
         self._stall_probe = None  # list of (event, event) pairs while exposed_comm_probe() is active
@@ -278,9 +278,9 @@ class FSDPViT:
     def exposed_comm_probe(self):
         """``with model.exposed_comm_probe() as r: <steps>`` -> r["ms"] = total time the compute stream spent
         blocked on communication-stream events (all-gather not there yet, reduce-scatter still reading a gradient
-        buffer, end-of-step join) and r["waits"] = number of such waits.  This is BASELINE.json's secondary metric
-        "exposed comm ms/step".  Two back-to-back event records cost ~2 us themselves, so ~0.3 ms per ViT-10B step
-        is measurement floor.  The all-gather slices pulled *inside* the qkv / fc1 GEMMs do not appear here: any
+        buffer, end-of-step join) and r["waits"] = number of such waits.  This is BASELINE.md's secondary metric
+        "exposed comm ms/step".  Event records cost time themselves, so a few tenths of a millisecond per
+        ViT-10B step are the measurement floor.  The all-gather slices pulled *inside* the qkv / fc1 GEMMs do not appear here: any
         stall there is part of that GEMM's duration."""
         res = {"ms": 0.0, "waits": 0}
         self._stall_probe = []

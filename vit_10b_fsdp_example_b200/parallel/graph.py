@@ -1,7 +1,7 @@
 """Whole-training-step CUDA graph.
 
 On XLA the reference's Python only *traces* a step and the compiled graph is launched once per iteration
-(run_vit_training.py:253 "the first few iterations are very slow due to compilation", SURVEY §3.3).  The CUDA
+(run_vit_training.py:253 "the first few iterations are very slow due to compilation").  The CUDA
 analogue is stream capture: forward, loss, backward (with recompute), the gathers / reduce-scatters on the
 communication stream, gradient clipping and the fused AdamW kernels are recorded once and replayed with a single
 launch per step.  For launch-bound models (ViT-L and smaller) this removes the ~1000 host launches per step.

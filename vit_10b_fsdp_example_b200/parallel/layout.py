@@ -5,7 +5,7 @@ run_vit_training.py:177-181): every parameter -- or, with ``--flatten_parameters
 flat parameter per unit -- is flattened, zero-padded to a multiple of the world size and chunked; a rank
 keeps only its chunk.
 
-B200-first layout: a unit owns ONE contiguous *full* buffer (what the GEMMs read through TMA) and ONE
+H100-first layout: a unit owns ONE contiguous *full* buffer (what the GEMMs read through TMA) and ONE
 contiguous *shard* buffer per rank.  The full buffer is a sequence of **shard groups**; group ``g`` spans
 ``world * g.shard_len`` elements and rank ``r`` owns the r-th ``shard_len`` slice of it:
 

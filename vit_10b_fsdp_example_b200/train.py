@@ -1,4 +1,4 @@
-"""Training driver on the B200-native engine.
+"""Training driver on the H100-native engine.
 
 Capability parity with the reference's driver (run_vit_training.py:203-324): datasets -> sharded model -> AdamW +
 warmup-cosine schedule -> optional resume -> epochs of [step, log every ``log_step_interval`` steps] -> per-rank

@@ -1,4 +1,4 @@
-"""Windowed meters and device timers (reference: utils.py:60-102 SmoothedValue; SURVEY §5.1/§5.5)."""
+"""Windowed meters and device timers (reference: utils.py:60-102 SmoothedValue)."""
 from __future__ import annotations
 
 import statistics
