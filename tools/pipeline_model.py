@@ -764,6 +764,180 @@ def model_gemm(seed: int, tiles: int, clusters: int = 2, num_kb: int = 3, stages
                     raise ProtocolError(f"tile {t} processed {done_tiles.get((t, c, w), 0)} times by epilogue warp {c}/{w}")
     return s
 
+
+# ---------------------------------------------------------------------------------------------------------------
+# gemm_sm90.cu with kClusterM = 2: CTA pairs along M, B tile multicast, static persistent schedule
+# ---------------------------------------------------------------------------------------------------------------
+class _CtaBar(TxBar):
+    """An mbarrier in one CTA's shared memory: arriving on it or completing bytes on it after that CTA exited is a
+    fault (the smem may already belong to another CTA)."""
+
+    def __init__(self, name: str, count: int, cta: dict):
+        super().__init__(name, count)
+        self.cta = cta
+
+    def arrive(self):
+        if self.cta["exited"]:
+            raise ProtocolError(f"{self.name}: arrival after its CTA exited")
+        super().arrive()
+
+    def complete_tx(self, n: int):
+        if self.cta["exited"]:
+            raise ProtocolError(f"{self.name}: bytes landed after its CTA exited")
+        super().complete_tx(n)
+
+
+def model_gemm_sm90_pair(seed: int, m_tiles: int, n_tiles: int, batch: int = 1, clusters: int = 2, num_kb: int = 3,
+                         stages: int = 3, bug: str = ""):
+    """`clusters` resident 2-CTA clusters walk units u = cluster, cluster + clusters, ... of m_units x n_tiles x batch
+    (m_units = ceil(m_tiles / 2)); CTA c of a cluster computes m-tile 2 mu + c (with odd m_tiles the last pair's second
+    CTA computes a tile below the matrix and still runs the whole protocol).  Per CTA: one TMA producer (expect_tx of
+    the whole stage on its own full barrier, its A tile to itself, its B half multicast to both CTAs, each copy
+    completing bytes on the receiving CTA's full barrier) and two consumer warpgroups (wgmma reads of A and both B
+    halves, one k-block in flight, each of their 4 warps releasing the stage on both CTAs' empty barriers of 16
+    arrivals); every thread meets the final cluster sync before its CTA exits.
+
+    Checked: liveness; every wgmma reads the k-block it expects in all three parts of its stage; no part of a stage is
+    overwritten while a read is outstanding; no barrier of an exited CTA is touched; every real tile is computed once
+    by each warpgroup.  bug = "local_only" (consumers release only their own CTA's stage, barriers counting 8) |
+    "no_final_sync" | "wait_peer_full" (a producer waits for the peer's full barrier instead of its own empty one)."""
+    s = Sim(seed)
+    A_BYTES, B_HALF = 2, 1  # bytes per stage part, in arbitrary units
+    m_units = (m_tiles + 1) // 2
+    per_batch = m_units * n_tiles
+    total = per_batch * batch
+    done: Dict[tuple, int] = {}
+    ctas = []
+
+    def tagged(name):
+        b = s.buf(name)
+        b.tag = None
+        return b
+
+    def build(cl):
+        pre = f"c{cl}."
+        cta = [{"exited": False, "live": 3} for _ in range(2)]  # producer + 2 consumer warpgroups
+        ctas.extend(cta)
+        empty_count = 4 * 2 * (1 if bug == "local_only" else 2)
+        full = [[_CtaBar(pre + f"full{c}_{i}", 1, cta[c]) for i in range(stages)] for c in range(2)]
+        empty = [[_CtaBar(pre + f"empty{c}_{i}", empty_count, cta[c]) for i in range(stages)] for c in range(2)]
+        for row in full + empty:
+            for b in row:
+                s.bars[b.name] = b
+        sa = [[tagged(pre + f"a{c}_{i}") for i in range(stages)] for c in range(2)]
+        sb = [[[tagged(pre + f"b{c}_{i}_h{h}") for h in range(2)] for i in range(stages)] for c in range(2)]
+        exit_sync = s.bar(pre + "cluster_sync", 6)
+        units = list(range(cl, total, clusters))
+
+        def teardown(c):
+            if bug != "no_final_sync":
+                yield ("arrive", exit_sync)
+                yield ("wait", exit_sync, 0)
+            yield ("exit", cta[c])
+
+        def producer(c):
+            stage = phase = 0
+            for u in units:
+                for kb in range(num_kb):
+                    if bug == "wait_peer_full":
+                        yield ("wait", full[1 - c][stage], phase ^ 1)
+                    else:
+                        yield ("wait", empty[c][stage], phase ^ 1)
+                    yield ("expect_tx", full[c][stage], A_BYTES + 2 * B_HALF)
+                    yield ("load", [(sa[c][stage], full[c][stage])], A_BYTES, (u, kb))
+                    yield ("load", [(sb[d][stage][c], full[d][stage]) for d in range(2)], B_HALF, (u, kb))
+                    stage = 0 if stage + 1 == stages else stage + 1
+                    phase ^= 1 if stage == 0 else 0
+            yield from teardown(c)
+
+        def release(c, st):
+            for _warp in range(4):
+                for d in ([c] if bug == "local_only" else [0, 1]):
+                    yield ("arrive", empty[d][st])
+
+        def consumer(c, w):
+            stage = phase = 0
+            groups: List[list] = []  # committed wgmma groups not yet retired
+            for u in units:
+                b, r = divmod(u, per_batch)
+                mu, nt = divmod(r, n_tiles)
+                prev = 0
+                for kb in range(num_kb):
+                    yield ("wait", full[c][stage], phase)
+                    yield ("wgmma", [sa[c][stage], sb[c][stage][0], sb[c][stage][1]], (u, kb), groups)
+                    if kb > 0:
+                        yield ("wgmma_wait", groups, 1)
+                        yield from release(c, prev)
+                    prev = stage
+                    stage = 0 if stage + 1 == stages else stage + 1
+                    phase ^= 1 if stage == 0 else 0
+                yield ("wgmma_wait", groups, 0)
+                yield from release(c, prev)
+                key = (b, 2 * mu + c, nt, w)
+                done[key] = done.get(key, 0) + 1
+            yield from teardown(c)
+
+        for c in range(2):
+            s.threads[pre + f"producer{c}"] = producer(c)
+            for w in range(2):
+                s.threads[pre + f"wg{c}_{w}"] = consumer(c, w)
+
+    for cl_ in range(clusters):
+        build(cl_)
+
+    base_do = s.do
+
+    def do(who, act):
+        kind = act[0]
+        if kind == "expect_tx":
+            act[1].expect_tx(act[2])
+        elif kind == "load":  # one TMA box, landing (independently) in each destination CTA
+            _, dests, nbytes, tag = act
+            for b, _bar in dests:
+                b.check_writable(who)
+                b.write_pending = True
+            for b, bar in dests:
+                def landed(b=b, bar=bar):
+                    b.write_pending = False
+                    b.version += 1
+                    b.tag = tag
+                    bar.complete_tx(nbytes)
+                s.tma_events.append(landed)
+        elif kind == "wgmma":
+            _, bufs, tag, groups = act
+            for b in bufs:
+                if b.write_pending:
+                    raise ProtocolError(f"{who}: {b.name} read while a TMA write is in flight")
+                if b.tag != tag:
+                    raise ProtocolError(f"{who}: {b.name} holds k-block {b.tag}, expected {tag}")
+                b.async_reads += 1
+            groups.append(bufs)
+        elif kind == "wgmma_wait":  # wgmma.wait_group N: all but the newest N groups have retired
+            _, groups, n = act
+            while len(groups) > n:
+                for b in groups.pop(0):
+                    b.async_reads -= 1
+        elif kind == "exit":
+            act[1]["live"] -= 1
+            if act[1]["live"] == 0:
+                act[1]["exited"] = True
+        else:
+            base_do(who, act)
+
+    s.do = do
+    s.run()
+    if not all(c["exited"] for c in ctas):
+        raise ProtocolError("a CTA never exited")
+    for b in range(batch):
+        for mt in range(m_tiles):
+            for nt in range(n_tiles):
+                for w in range(2):
+                    if done.get((b, mt, nt, w), 0) != 1:
+                        raise ProtocolError(f"tile {(b, mt, nt)} computed {done.get((b, mt, nt, w), 0)} times by "
+                                            f"warpgroup {w}")
+    return s
+
+
 if __name__ == "__main__":
     for seed in range(200):
         model_bwd(seed, 1, 4, 2, 4, True, False)
@@ -774,4 +948,5 @@ if __name__ == "__main__":
         model_fwd_persist(seed, 3, 4)  # softmax + separate epilogue warps (round-2 kernel)
         model_fwd_long(seed, 9)
         model_gemm(seed, 9, clusters=2, epi_warps=2)
+        model_gemm_sm90_pair(seed, 5, 3, batch=2, clusters=3)
     print("all protocols passed 200 schedules each")

@@ -34,7 +34,7 @@ inline cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().strea
 void gemm(Tensor a, int64_t lda, int64_t major_a, Tensor b, int64_t ldb, int64_t major_b, Tensor d, int64_t ldd,
           int64_t M, int64_t N, int64_t K, OptT bias, OptT residual, int64_t ld_res, int64_t res_row_mod, OptT aux_in,
           int64_t ld_aux, OptT aux_out, int64_t ld_aux_out, OptT colsum, int64_t colsum_bi_stride, int64_t act,
-          std::vector<int64_t> batch, int64_t block_n, int64_t max_ctas, std::vector<int64_t> ag) {
+          std::vector<int64_t> batch, int64_t block_n, int64_t cluster, int64_t max_ctas, std::vector<int64_t> ag) {
     c10::cuda::CUDAGuard guard(a.device());
     b200::GemmOperand A, B, D, X;
     A.ptr = bf16_ptr(a), A.ld = lda;
@@ -69,7 +69,7 @@ void gemm(Tensor a, int64_t lda, int64_t major_a, Tensor b, int64_t ldb, int64_t
         for (int64_t r = 0; r < ag[0]; ++r) fuse.peer_src[r] = static_cast<uint64_t>(ag[6 + r]);
     }
     b200::gemm_bf16(A, (int)major_a, B, (int)major_b, D, aux_out.has_value() ? &X : nullptr, (int)M, (int)N, (int)K, e,
-                    (int)block_n, (int)max_ctas, cur_stream(), ag.empty() ? nullptr : &fuse);
+                    (int)block_n, (int)cluster, (int)max_ctas, cur_stream(), ag.empty() ? nullptr : &fuse);
 }
 
 void layernorm_fwd(Tensor x, Tensor gamma, Tensor beta, Tensor y, Tensor mean, Tensor rstd, double eps) {

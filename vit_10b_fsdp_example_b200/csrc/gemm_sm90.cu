@@ -51,6 +51,7 @@ struct KernelParams {
     int M, N, K;
     int batch, nb_inner;
     int m_tiles, n_tiles;  // CTA tiles (128 x BLOCK_N)
+    int m_units;           // m-tiles per raster column: m_tiles, or m-tile pairs when CTAs run in 2-CTA clusters
     int n_rot;             // n-tile rotation so that tiles are visited in slab-arrival order (AG fusion)
     int group_n;           // n-tiles per raster group
     GemmEpilogue epi;
@@ -79,9 +80,17 @@ __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.pr
 
 // erf via Abramowitz-Stegun 7.1.26 (|err| < 1.5e-7, far below bf16 resolution): 1 rcp + 1 exp + 6 FMA.
 // e = exp(-z^2) is returned too: for z = x/sqrt(2) it is exactly the Gaussian factor gelu'(x) needs.
+__device__ __forceinline__ float rcp_approx(float x) {
+    float r;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+    return r;
+}
 __device__ __forceinline__ float erf_as(float z, float& e) {
     const float az = fabsf(z);
-    const float t = __frcp_rn(fmaf(0.3275911f, az, 1.0f));
+    // rcp.approx (relative error <= 2^-23, below the 1.5e-7 of the formula) rather than __frcp_rn: the correctly
+    // rounded reciprocal calls a slow-path subroutine, and the GEMM kernel must stay free of calls (see its body).
+    // The argument is >= 1, never in that slow range.
+    const float t = rcp_approx(fmaf(0.3275911f, az, 1.0f));
     e = __expf(-az * az);
     float poly = fmaf(1.061405429f, t, -1.453152027f);
     poly = fmaf(poly, t, 1.421413741f);
@@ -100,7 +109,18 @@ __device__ __forceinline__ float dgelu_erf(float x) {
     return fmaf(x * 0.3989422804014327f, e, cdf);  // cdf + x * pdf,  pdf = exp(-x^2/2)/sqrt(2 pi)
 }
 
-template <int kMajorA, int kMajorB, int BLOCK_N, int kStages>
+// kClusterM = 2: CTAs run in (2, 1, 1) clusters.  The two CTAs of a cluster own m-tiles 2 mp and 2 mp + 1 of the same
+// (batch, n-tile), so they need the same B tile: each producer loads its own A tile and one half of B, multicast to
+// both CTAs at the same stage offset.  Per k-block a CTA then pulls 16 KB of A + BLOCK_N / 2 rows of B from L2
+// instead of 16 KB + BLOCK_N rows.  Stage layout, descriptors and consumer code are the same as with kClusterM = 1;
+// only the barrier protocol changes:
+//   full_bar[s]  1 arrival (the local producer's expect_tx of the whole stage); the peer's B half completes its bytes
+//                here too, possibly before the local expect_tx (the tx count may dip below zero meanwhile).
+//   empty_bar[s] 8 * kClusterM arrivals: every consumer warp of BOTH CTAs arrives on both CTAs' barriers, because a
+//                producer's multicast writes stage s of the peer as well and may start only once both released it.
+// Both CTAs walk the same tile sequence, so they fill and drain the ring in lock step; cluster syncs after barrier
+// init and before exit keep a CTA from multicasting into, or arriving on, a peer that has not started or has left.
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM>
 __global__ void __launch_bounds__(kNumThreads, 1)
     gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                           const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_aux,
@@ -110,6 +130,7 @@ __global__ void __launch_bounds__(kNumThreads, 1)
     constexpr int kStageBytes = kABytes + kBBytes;
     static_assert(BLOCK_N % 64 == 0 && BLOCK_N <= 256, "epilogue works in 64-column chunks; wgmma N <= 256");
     static_assert(kABytes % 1024 == 0 && kBBytes % 1024 == 0, "swizzle-128B needs 1024 B aligned stages");
+    static_assert(kClusterM == 1 || (kClusterM == 2 && BLOCK_N % 128 == 0), "B splits into two 64-row multiples");
 
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* smem_cd = smem;
@@ -121,10 +142,9 @@ __global__ void __launch_bounds__(kNumThreads, 1)
     const uint32_t warp_idx = threadIdx.x / 32;
     const uint32_t lane = lane_id();
     const uint32_t wg = warp_idx / 4;  // 0: producer + all-gather copier, 1-2: consumers
-    if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) {  // SWIZZLE_128B tiles must start on a 1024-byte boundary
-        printf("[b200] gemm: dynamic shared memory is not 1024-byte aligned\n");
-        __trap();
-    }
+    // No printf anywhere in this kernel: a printf is a function call, and any call in a kernel that uses wgmma makes
+    // ptxas serialise every wgmma (warning C7510: each MMA then waits for the previous one).  Faults trap silently.
+    if (threadIdx.x == 0 && (smem_u32(smem) & 1023u) != 0) __trap();  // SWIZZLE_128B tiles need 1024-B alignment
 
     if (warp_idx == 0 && elect_one()) {
         prefetch_tmap(&tmap_a);
@@ -132,29 +152,40 @@ __global__ void __launch_bounds__(kNumThreads, 1)
         prefetch_tmap(&tmap_d);
         if (p.epi.has_aux_out) prefetch_tmap(&tmap_aux);
         for (int i = 0; i < kStages; ++i) {
-            mbar_init(&full_bar[i], 1);               // the producer's expect_tx arrive
-            mbar_init(&empty_bar[i], kConsumerWgs * 4);  // lane 0 of every consumer warp
+            mbar_init(&full_bar[i], 1);                              // the producer's expect_tx arrive
+            mbar_init(&empty_bar[i], kConsumerWgs * 4 * kClusterM);  // lane 0 of every consumer warp of the cluster
         }
         fence_mbar_init();
     }
-    __syncthreads();
+    if constexpr (kClusterM > 1)
+        cluster_sync();  // the peer's barriers are initialised before anything is multicast to or arrives on them
+    else
+        __syncthreads();
 
-    const int tiles_per_batch = p.m_tiles * p.n_tiles;
-    const int total_tiles = tiles_per_batch * p.batch;
+    // A unit is one tile (kClusterM = 1) or one cluster's pair of vertically adjacent tiles (kClusterM = 2).
+    // The rank is re-read from its special register where used: the consumers run at the register limit.
+    auto cta_rank = [] { return kClusterM > 1 ? static_cast<int>(cluster_ctarank()) : 0; };
+    const int units_per_batch = p.m_units * p.n_tiles;
+    const int total_units = units_per_batch * p.batch;
     const int num_kb = (p.K + kBlockK - 1) / kBlockK;
     const int kGroupN = p.group_n;  // n-tiles per raster group (keeps a wave's A/B footprint L2-resident)
 
-    // Static persistent schedule: CTA c computes tiles c, c + grid, c + 2 grid, ...  The tiles in flight are a
-    // contiguous window of the raster, so co-running CTAs share A / B panels in L2.
+    // Static persistent schedule: CTA (or cluster) c computes units c, c + grid, c + 2 grid, ...  The units in flight
+    // are a contiguous window of the raster, so co-running CTAs share A / B panels in L2.
+    // With an odd m-tile count the second CTA of the last pair gets m-tile m_tiles, wholly below the matrix.  It still
+    // runs the full protocol (its B half feeds the peer, its consumers release the peer's stages).  Its A box is
+    // wholly out of bounds: TMA fills it with zeros and still counts its bytes (the kernel relies on that already for
+    // the out-of-range 64-row boxes of MN-major operands), and its output rows are clipped by the TMA store and zeroed
+    // for the column sums like any row >= M.  Keeping the load avoids a second producer path for one tile per column.
     auto decode_tile = [&](int t, int& b, int& mt, int& nt) {
-        b = t / tiles_per_batch;
-        const int r = t - b * tiles_per_batch;
-        const int per_group = p.m_tiles * kGroupN;
+        b = t / units_per_batch;
+        const int r = t - b * units_per_batch;
+        const int per_group = p.m_units * kGroupN;
         const int g = r / per_group;
         const int first_n = g * kGroupN;
         const int gsz = min(kGroupN, p.n_tiles - first_n);
         const int in_g = r - g * per_group;
-        mt = in_g / gsz;
+        mt = (in_g / gsz) * kClusterM + cta_rank();
         nt = first_n + in_g % gsz;
         nt += p.n_rot;  // AG fusion: start with the n-tiles of the locally owned slab
         if (nt >= p.n_tiles) nt -= p.n_tiles;
@@ -168,7 +199,7 @@ __global__ void __launch_bounds__(kNumThreads, 1)
             // ================================= TMA producer =================================
             if (elect_one()) {
                 uint32_t stage = 0, phase = 0;
-                for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+                for (int t = blockIdx.x / kClusterM; t < total_units; t += gridDim.x / kClusterM) {
                     int b, mt, nt;
                     decode_tile(t, b, mt, nt);
                     const int bi = b % p.nb_inner, bo = b / p.nb_inner;
@@ -183,17 +214,14 @@ __global__ void __launch_bounds__(kNumThreads, 1)
                             for (int sl = s_lo; sl <= s_hi; ++sl) {
                                 uint32_t spins = 0;
                                 while (ld_acquire_gpu(p.ag.flags + sl) < static_cast<uint32_t>(ag_chunks_per_slab)) {
-                                    if (++spins > (1u << 26)) {
-                                        printf("[b200] AG-fused GEMM: slab %d never arrived (block %d)\n", sl, blockIdx.x);
-                                        __trap();
-                                    }
+                                    if (++spins > (1u << 26)) __trap();  // slab never arrived
                                 }
                             }
                             fence_proxy_async_all();  // generic-proxy peer copies -> async-proxy (TMA) reads
                         }
                     }
                     for (int kb = 0; kb < num_kb; ++kb) {
-                        mbar_wait(&empty_bar[stage], phase ^ 1);
+                        mbar_wait_silent(&empty_bar[stage], phase ^ 1);
                         const int k_idx = kb * kBlockK;
                         uint8_t* sa = smem_a + stage * kABytes;
                         uint8_t* sb = smem_b + stage * kBBytes;
@@ -206,13 +234,31 @@ __global__ void __launch_bounds__(kNumThreads, 1)
                                 tma_load_4d(&tmap_a, &full_bar[stage], sa + i * (64 * kBlockK * 2), m_idx + i * 64,
                                                  k_idx, bi, bo);
                         }
-                        if constexpr (kMajorB == 0) {
-                            tma_load_4d(&tmap_b, &full_bar[stage], sb, k_idx, n_idx, bi, bo);
-                        } else {
+                        if constexpr (kClusterM == 1) {
+                            if constexpr (kMajorB == 0) {
+                                tma_load_4d(&tmap_b, &full_bar[stage], sb, k_idx, n_idx, bi, bo);
+                            } else {
 #pragma unroll
-                            for (int i = 0; i < BLOCK_N / 64; ++i)
-                                tma_load_4d(&tmap_b, &full_bar[stage], sb + i * (64 * kBlockK * 2), n_idx + i * 64,
-                                                 k_idx, bi, bo);
+                                for (int i = 0; i < BLOCK_N / 64; ++i)
+                                    tma_load_4d(&tmap_b, &full_bar[stage], sb + i * (64 * kBlockK * 2), n_idx + i * 64,
+                                                k_idx, bi, bo);
+                            }
+                        } else {
+                            // this CTA's half of B: rows [n_idx + h, n_idx + h + BLOCK_N / 2), h = rank * BLOCK_N / 2,
+                            // to stage offset h * 128 B in both CTAs (the (64, BLOCK_N / 2) box of a K-major B is
+                            // laid out exactly like the lower or upper half of the (64, BLOCK_N) box)
+                            constexpr int kHalfN = BLOCK_N / 2;
+                            const int h = cta_rank() * kHalfN;
+                            if constexpr (kMajorB == 0) {
+                                tma_load_4d_multicast(&tmap_b, &full_bar[stage], sb + h * (kBlockK * 2), k_idx,
+                                                      n_idx + h, bi, bo, 0b11);
+                            } else {
+#pragma unroll
+                                for (int i = 0; i < kHalfN / 64; ++i)
+                                    tma_load_4d_multicast(&tmap_b, &full_bar[stage],
+                                                          sb + (h / 64 + i) * (64 * kBlockK * 2), n_idx + h + i * 64,
+                                                          k_idx, bi, bo, 0b11);
+                            }
                         }
                         stage = (stage + 1 == kStages) ? 0 : stage + 1;
                         phase ^= (stage == 0);
@@ -274,8 +320,17 @@ __global__ void __launch_bounds__(kNumThreads, 1)
         uint32_t stage = 0, phase = 0;
         uint32_t flip = 0;
         float d[BLOCK_N / 2];
+        // hand stage s back to the producers that write it: this CTA's, and with multicast the peer's too
+        auto release = [&](uint32_t s) {
+            if constexpr (kClusterM == 1) {
+                mbar_arrive(&empty_bar[s]);
+            } else {
+#pragma unroll
+                for (int c = 0; c < kClusterM; ++c) mbar_arrive_cluster(&empty_bar[s], c);
+            }
+        };
 
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+        for (int t = blockIdx.x / kClusterM; t < total_units; t += gridDim.x / kClusterM) {
             int b, mt, nt;
             decode_tile(t, b, mt, nt);
             const int bi = b % p.nb_inner, bo = b / p.nb_inner;
@@ -284,7 +339,7 @@ __global__ void __launch_bounds__(kNumThreads, 1)
 
             uint32_t prev_stage = 0;
             for (int kb = 0; kb < num_kb; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
+                mbar_wait_silent(&full_bar[stage], phase);
                 const uint32_t a_addr = smem_u32(smem_a + stage * kABytes) + cw * kSlabA;
                 const uint32_t b_addr = smem_u32(smem_b + stage * kBBytes);
                 wgmma_fence();
@@ -297,14 +352,14 @@ __global__ void __launch_bounds__(kNumThreads, 1)
                 wgmma_commit();
                 if (kb > 0) {
                     wgmma_wait<1>();  // the previous k-block's MMAs are done reading their slot
-                    if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+                    if (lane == 0) release(prev_stage);
                 }
                 prev_stage = stage;
                 stage = (stage + 1 == kStages) ? 0 : stage + 1;
                 phase ^= (stage == 0);
             }
             wgmma_wait<0>();
-            if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+            if (lane == 0) release(prev_stage);
 
             // ---- epilogue: registers -> swizzled staging buffer -> TMA store, 64 columns at a time ----
             const int row0 = m0 + static_cast<int>(wrow), row1 = row0 + 8;
@@ -398,6 +453,12 @@ __global__ void __launch_bounds__(kNumThreads, 1)
             }
         }
         if (etid == 0) tma_store_wait<0>();
+    }
+    if constexpr (kClusterM > 1) {
+        // the peer's last multicasts into this CTA have landed (our consumers waited for them), but its consumers may
+        // still be about to arrive on our empty barriers: leave only together
+        __syncwarp();
+        cluster_sync();
     }
 }
 
@@ -497,21 +558,48 @@ int num_sms() {
     return n;
 }
 
-template <int kMajorA, int kMajorB, int BLOCK_N, int kStages>
+void check(cudaError_t err, const char* what) {
+    if (err != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(err));
+}
+
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM>
 void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, const GemmOperand* aux, int M, int N,
             int K, const GemmEpilogue& epi, int max_ctas, cudaStream_t stream, const GemmAgFuse* ag) {
     constexpr int kSmem = kCdBufs * kCdBufBytes + kStages * (kBlockM + BLOCK_N) * kBlockK * 2 + 2 * kStages * 8;
     static_assert(kSmem <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
-    auto kern = gemm_bf16_sm90_kernel<kMajorA, kMajorB, BLOCK_N, kStages>;
+    auto kern = gemm_bf16_sm90_kernel<kMajorA, kMajorB, BLOCK_N, kStages, kClusterM>;
     static bool attr_set = false;
     if (!attr_set) {
-        cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-        if (err != cudaSuccess) throw std::runtime_error(std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(err));
+        check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem), "cudaFuncSetAttribute");
         attr_set = true;
     }
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute cluster_attr;
+    cluster_attr.id = cudaLaunchAttributeClusterDimension;
+    cluster_attr.val.clusterDim.x = kClusterM, cluster_attr.val.clusterDim.y = 1, cluster_attr.val.clusterDim.z = 1;
+    cfg.blockDim = dim3(kNumThreads);
+    cfg.dynamicSmemBytes = kSmem;
+    cfg.stream = stream;
+    cfg.attrs = &cluster_attr;
+    cfg.numAttrs = kClusterM > 1 ? 1 : 0;
+    // Clusters that can be resident at once: a cluster's CTAs must share a GPC, so with one CTA per SM this can be
+    // fewer than num_sms / 2.  The schedule is a static stride over a persistent grid, so one cluster more than fits
+    // would run as a second wave after the first and about double the GEMM's time.
+    static int resident_units = 0;
+    if (resident_units == 0) {
+        if constexpr (kClusterM == 1) {
+            resident_units = num_sms();
+        } else {
+            cfg.gridDim = dim3(num_sms() / kClusterM * kClusterM);
+            check(cudaOccupancyMaxActiveClusters(&resident_units, kern, &cfg), "cudaOccupancyMaxActiveClusters");
+            if (resident_units < 1) throw std::runtime_error("gemm: no 2-CTA cluster of this kernel fits an SM pair");
+        }
+    }
     // A: K-major -> (inner=K, outer=M), box (64, 128).  MN-major -> (inner=M, outer=K), box (64, 64).
+    // B: K-major -> box (64, BLOCK_N / kClusterM): each CTA of a cluster loads its share.  MN-major -> box (64, 64).
     CUtensorMap ta = kMajorA == 0 ? make_tmap(A, K, M, kBlockK, kBlockM) : make_tmap(A, M, K, 64, kBlockK);
-    CUtensorMap tb = kMajorB == 0 ? make_tmap(B, K, N, kBlockK, BLOCK_N) : make_tmap(B, N, K, 64, kBlockK);
+    CUtensorMap tb =
+        kMajorB == 0 ? make_tmap(B, K, N, kBlockK, BLOCK_N / kClusterM) : make_tmap(B, N, K, 64, kBlockK);
     CUtensorMap td = make_tmap(D, N, M, 64, 64);
     CUtensorMap tx = (epi.has_aux_out && aux != nullptr) ? make_tmap(*aux, N, M, 64, 64) : td;
 
@@ -520,6 +608,7 @@ void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, co
     p.batch = static_cast<int>(D.nb_inner * D.nb_outer);
     p.nb_inner = static_cast<int>(D.nb_inner);
     p.m_tiles = (M + kBlockM - 1) / kBlockM;
+    p.m_units = (p.m_tiles + kClusterM - 1) / kClusterM;
     p.n_tiles = (N + BLOCK_N - 1) / BLOCK_N;
     p.epi = epi;
     p.n_rot = 0;
@@ -535,13 +624,13 @@ void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, co
         p.n_rot = static_cast<int>((static_cast<int64_t>(ag->rank) * ag->rows_per_slab) / BLOCK_N) % p.n_tiles;
         cudaMemsetAsync(ag->flags, 0, sizeof(uint32_t) * (ag->world + 1), stream);  // slab counters + chunk counter
     }
-    const int64_t total = static_cast<int64_t>(p.m_tiles) * p.n_tiles * p.batch;
-    int sms = num_sms();
-    if (max_ctas > 0 && max_ctas < sms) sms = max_ctas;
-    const int ctas = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(total, sms)));
-    kern<<<ctas, kNumThreads, kSmem, stream>>>(ta, tb, td, tx, p);
-    cudaError_t err = cudaGetLastError();
-    if (err != cudaSuccess) throw std::runtime_error(std::string("gemm launch failed: ") + cudaGetErrorString(err));
+    const int64_t total = static_cast<int64_t>(p.m_units) * p.n_tiles * p.batch;
+    int units = resident_units;
+    if (max_ctas > 0) units = std::min(units, max_ctas / kClusterM);  // max_ctas >= kClusterM (gemm_bf16)
+    units = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(total, units)));
+    cfg.gridDim = dim3(units * kClusterM);
+    check(cudaLaunchKernelEx(&cfg, kern, ta, tb, td, tx, p), "gemm launch failed");
+    check(cudaGetLastError(), "gemm launch failed");
 }
 
 }  // namespace
@@ -552,18 +641,24 @@ CUtensorMap make_tensor_map_4d(const GemmOperand& op, int64_t inner, int64_t out
 }
 
 void gemm_bf16(const GemmOperand& A, int major_a, const GemmOperand& B, int major_b, const GemmOperand& D,
-               const GemmOperand* aux_out, int M, int N, int K, const GemmEpilogue& epi, int block_n, int max_ctas,
-               cudaStream_t stream, const GemmAgFuse* ag) {
+               const GemmOperand* aux_out, int M, int N, int K, const GemmEpilogue& epi, int block_n, int cluster,
+               int max_ctas, cudaStream_t stream, const GemmAgFuse* ag) {
     if (N % 8 != 0 && (epi.residual || epi.aux_in))
         throw std::runtime_error("gemm: N must be a multiple of 8 when residual/aux_in are used");
     if (epi.act == kActDGelu && (epi.residual != nullptr || epi.aux_in == nullptr))
         throw std::runtime_error("gemm: dGELU epilogue needs aux_in and cannot be combined with a residual");
     if (D.nb_inner * D.nb_outer > 1 && (epi.bias || epi.residual || epi.aux_in))
         throw std::runtime_error("gemm: bias/residual/aux_in are not supported for batched problems");
+    if (cluster != 0 && cluster != 1 && cluster != 2) throw std::runtime_error("gemm: cluster must be 0 (auto), 1 or 2");
     if (block_n == 0) block_n = (N > 128) ? 256 : 128;
+    // Auto is one CTA per tile: CTA pairs are no faster on the ViT-10B block GEMMs (measurements in DESIGN.md).
+    if (cluster == 0 || max_ctas == 1) cluster = 1;
 #define B200_DISPATCH(MA, MB, BN, ST)                                                             \
     if (major_a == MA && major_b == MB && block_n == BN) {                                        \
-        launch<MA, MB, BN, ST>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);             \
+        if (cluster == 2)                                                                         \
+            launch<MA, MB, BN, ST, 2>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);      \
+        else                                                                                      \
+            launch<MA, MB, BN, ST, 1>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);      \
         return;                                                                                   \
     }
     B200_DISPATCH(0, 0, 256, 4)

@@ -48,10 +48,11 @@ struct GemmAgFuse {
 };
 
 // D[b][M, N] = epi(A[b] (M x K) * B[b] (N x K)^T).  major_x: 0 = K contiguous, 1 = M/N contiguous.
-// block_n: 0 = auto, else 128 / 256.  max_ctas: 0 = all SMs (used to carve SMs out for comm kernels).
+// block_n: 0 = auto, else 128 / 256.  cluster: 0 = auto (= 1), 1 = one CTA per tile, 2 = CTA pairs along M sharing
+// B through TMA multicast (1 is used when max_ctas = 1).  max_ctas: 0 = all SMs (used to carve SMs out for comm kernels).
 void gemm_bf16(const GemmOperand& A, int major_a, const GemmOperand& B, int major_b, const GemmOperand& D,
-               const GemmOperand* aux_out, int M, int N, int K, const GemmEpilogue& epi, int block_n, int max_ctas,
-               cudaStream_t stream, const GemmAgFuse* ag = nullptr);
+               const GemmOperand* aux_out, int M, int N, int K, const GemmEpilogue& epi, int block_n, int cluster,
+               int max_ctas, cudaStream_t stream, const GemmAgFuse* ag = nullptr);
 
 // Cached 4-D bf16 TMA descriptor: dims (inner, outer, op.nb_inner, op.nb_outer), box (box_inner, box_outer, 1, 1).
 CUtensorMap make_tensor_map_4d(const GemmOperand& op, int64_t inner, int64_t outer, int box_inner, int box_outer,

@@ -117,6 +117,15 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
     }
 }
 
+// The same bounded wait without the diagnostic printf, for kernels that issue wgmma: a printf is a function call, and
+// any call in such a kernel makes ptxas serialise every wgmma (warning C7510: each MMA waits for the previous one).
+__device__ __forceinline__ void mbar_wait_silent(uint64_t* bar, uint32_t phase) {
+    uint32_t spins = 0;
+    while (!mbar_try_wait(bar, phase)) {
+        if (++spins > B200_SPIN_LIMIT) __trap();
+    }
+}
+
 // ----------------------------------------------------------------------------------------------
 // TMA
 // ----------------------------------------------------------------------------------------------
@@ -131,6 +140,17 @@ __device__ __forceinline__ void tma_load_4d(const void* tmap, uint64_t* bar, voi
         "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes"
         " [%0], [%1, {%3, %4, %5, %6}], [%2];" ::"r"(smem_u32(smem)),
         "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+        : "memory");
+}
+
+// 4-D tiled load multicast to every CTA of the cluster in `cta_mask`: the box lands at the same smem offset in each
+// of them and completes bytes on the mbarrier at `bar`'s offset in each of them.
+__device__ __forceinline__ void tma_load_4d_multicast(const void* tmap, uint64_t* bar, void* smem, int c0, int c1,
+                                                      int c2, int c3, uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4, %5, %6}], [%2], %7;" ::"r"(smem_u32(smem)),
+        "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "h"(cta_mask)
         : "memory");
 }
 

@@ -76,6 +76,16 @@ def set_compute_max_ctas(n: int) -> None:
     _max_ctas = int(n)
 
 
+# GEMM CTA-cluster size: 0 = auto (one CTA per tile, see gemm_bf16), 1 or 2 (CTA pairs sharing the B tile) forced.
+_gemm_cluster = 0
+
+
+def set_gemm_cluster(n: int) -> None:
+    global _gemm_cluster
+    assert n in (0, 1, 2), n
+    _gemm_cluster = int(n)
+
+
 def _ld(t: torch.Tensor) -> int:
     assert t.dim() == 2 and t.stride(1) == 1, "expected a row-major 2-D (possibly strided) matrix"
     return t.stride(0)
@@ -107,10 +117,10 @@ def _bias_ok(b: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
 
 def gemm_raw(a, lda, major_a, b, ldb, major_b, d, ldd, M, N, K, *, bias=None, residual=None, ld_res=0,
              res_row_mod=0, aux_in=None, ld_aux=0, aux_out=None, ld_aux_out=0, colsum=None, colsum_bi_stride=0,
-             act=ACT_NONE, batch=(), block_n=0, max_ctas=None, ag=()):
+             act=ACT_NONE, batch=(), block_n=0, cluster=None, max_ctas=None, ag=()):
     _C.gemm(a, lda, major_a, b, ldb, major_b, d, ldd, M, N, K, bias, residual, ld_res, res_row_mod, aux_in, ld_aux,
             aux_out, ld_aux_out, colsum, colsum_bi_stride, act, list(batch), block_n,
-            _max_ctas if max_ctas is None else max_ctas, list(ag))
+            _gemm_cluster if cluster is None else cluster, _max_ctas if max_ctas is None else max_ctas, list(ag))
 
 
 # ------------------------------------------------------------------------------------------------
