@@ -20,7 +20,8 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 BUILD_DIR = os.path.join(CSRC, "build")
 SO_PATH = os.path.join(PKG_DIR, "_C.so")
 
-CU_SOURCES = ["gemm_sm90.cu", "elementwise.cu", "comm.cu", "attention_sm90.cu", "layernorm_stream.cu"]
+CU_SOURCES = ["gemm_sm90.cu", "elementwise.cu", "comm.cu", "attention_sm90.cu", "attention_drop_sm90.cu",
+              "layernorm_stream.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 
 NVCC_FLAGS = [

@@ -101,17 +101,20 @@ void softmax_bwd(Tensor dp, Tensor p, int64_t rows, int64_t n, int64_t ld, doubl
 
 bool attention_supported(int64_t N, int64_t hd) { return b200::attention_supported((int)N, (int)hd); }
 
-void attention_fwd(Tensor qkv, Tensor out, OptT lse, OptT probs, int64_t B, int64_t N, int64_t H, int64_t hd) {
+// drop_p > 0: attention dropout with the mask `dropout` draws for drop_key over [B*H, N, pad8(N)] probabilities.
+void attention_fwd(Tensor qkv, Tensor out, OptT lse, OptT probs, int64_t B, int64_t N, int64_t H, int64_t hd,
+                   double drop_p, int64_t drop_key) {
     c10::cuda::CUDAGuard guard(qkv.device());
     TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && out.is_contiguous(), "attention_fwd: bad layouts");
     TORCH_CHECK(!lse.has_value() || (lse->is_contiguous() && lse->numel() == B * H * N), "attention_fwd: bad lse");
+    TORCH_CHECK(drop_p == 0.0 || !probs.has_value(), "attention_fwd: no probability output with dropout");
     b200::attention_fwd(bf16_ptr(qkv), qkv.stride(0), bf16_mut(out), lse.has_value() ? f32_ptr(*lse) : nullptr,
                         probs.has_value() ? bf16_mut(*probs) : nullptr, probs.has_value() ? probs->size(2) : 0, (int)B,
-                        (int)N, (int)H, (int)hd, cur_stream());
+                        (int)N, (int)H, (int)hd, cur_stream(), (float)drop_p, (uint64_t)drop_key);
 }
 
 void attention_bwd(Tensor qkv, Tensor dout, Tensor out, Tensor lse, Tensor delta, Tensor dqkv, OptT colsum, int64_t B,
-                   int64_t N, int64_t H, int64_t hd) {
+                   int64_t N, int64_t H, int64_t hd, double drop_p, int64_t drop_key) {
     c10::cuda::CUDAGuard guard(qkv.device());
     TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && dout.stride(1) == 1 && out.stride(1) == 1 &&
                     dqkv.is_contiguous() && lse.is_contiguous() && delta.is_contiguous(),
@@ -120,7 +123,7 @@ void attention_bwd(Tensor qkv, Tensor dout, Tensor out, Tensor lse, Tensor delta
                 "attention_bwd: bad shapes");
     b200::attention_bwd(bf16_ptr(qkv), qkv.stride(0), bf16_ptr(dout), dout.stride(0), bf16_ptr(out), out.stride(0),
                         f32_ptr(lse), f32_ptr(delta), bf16_mut(dqkv), (int)B, (int)N, (int)H, (int)hd, cur_stream(),
-                        colsum.has_value() ? f32_ptr(*colsum) : nullptr);
+                        colsum.has_value() ? f32_ptr(*colsum) : nullptr, (float)drop_p, (uint64_t)drop_key);
 }
 
 void cross_entropy(Tensor logits, Tensor target, OptT dlogits, Tensor loss, OptT correct) {
@@ -319,9 +322,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("layernorm_bwd", &layernorm_bwd);
     m.def("softmax_fwd", &softmax_fwd);
     m.def("softmax_bwd", &softmax_bwd);
-    m.def("attention_fwd", &attention_fwd);
+    namespace py = pybind11;
+    m.def("attention_fwd", &attention_fwd, py::arg("qkv"), py::arg("out"), py::arg("lse"), py::arg("probs"), py::arg("B"),
+          py::arg("N"), py::arg("H"), py::arg("hd"), py::arg("drop_p") = 0.0, py::arg("drop_key") = 0);
     m.def("attention_supported", &attention_supported);
-    m.def("attention_bwd", &attention_bwd);
+    m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("dout"), py::arg("out"), py::arg("lse"),
+          py::arg("delta"), py::arg("dqkv"), py::arg("colsum"), py::arg("B"), py::arg("N"), py::arg("H"), py::arg("hd"),
+          py::arg("drop_p") = 0.0, py::arg("drop_key") = 0);
     m.def("cross_entropy", &cross_entropy);
     m.def("im2col", &im2col);
     m.def("gelu_fwd", &gelu_fwd);

@@ -18,6 +18,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "dropout.cuh"
 #include "elementwise.h"
 #include "ptx.cuh"
 
@@ -477,24 +478,9 @@ __global__ void __launch_bounds__(256) dgelu_mul_kernel(const __nv_bfloat16* __r
 // 345-347): y = x * keep / (1 - p) with keep drawn from Philox-4x32-10, counter = index of the 16-byte vector, key =
 // the 64-bit (seed, step, site) key of the engine's DropoutCtx.  The mask is a pure function of (key, element index),
 // so the activation-checkpoint recompute and the backward pass regenerate it instead of storing it: one Philox call
-// yields 8 x 16 random bits = the 8 bf16 values of a vector (keep <=> r16 >= p * 65536).
+// yields 8 x 16 random bits = the 8 bf16 values of a vector (keep <=> r16 >= p * 65536).  philox4x32_10 and the
+// threshold live in dropout.cuh: the fused attention kernels regenerate the same mask for attention dropout.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t k0, uint32_t k1, uint32_t (&out)[4]) {
-    uint32_t c2 = 0x5eed5eedu, c3 = 0x0b200b20u;
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-        c0 = hi1 ^ c1 ^ k0;
-        c1 = lo1;
-        c2 = hi0 ^ c3 ^ k1;
-        c3 = lo0;
-        k0 += 0x9E3779B9u;
-        k1 += 0xBB67AE85u;
-    }
-    out[0] = c0, out[1] = c1, out[2] = c2, out[3] = c3;
-}
-
 __global__ void __launch_bounds__(256) dropout_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
                                                       int64_t nvec, uint32_t key_lo, uint32_t key_hi, uint32_t thresh16,
                                                       float scale) {
@@ -1044,9 +1030,9 @@ void dropout(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, float p, uint6
     if (!(p >= 0.f && p < 1.f)) throw std::runtime_error("dropout: p must be in [0, 1)");
     const int grid = static_cast<int>(std::min<int64_t>((n / 8 + 255) / 256, sm_count() * 16));
     if (grid == 0) return;
-    const uint32_t thresh = static_cast<uint32_t>(p * 65536.0f + 0.5f);
+    const uint32_t thresh = dropout_thresh16(p);
     dropout_kernel<<<grid, 256, 0, stream>>>(x, y, n / 8, static_cast<uint32_t>(key), static_cast<uint32_t>(key >> 32),
-                                            thresh, 1.0f / (1.0f - static_cast<float>(thresh) / 65536.0f));
+                                            thresh, dropout_scale(thresh));
     check_launch("dropout");
 }
 

@@ -141,7 +141,14 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     lse = None
     if use_drop and pa > 0:
         masks["att"] = drop.key(site + 0)
-        a, P = ops.attention_fwd(qkv, B, N, H, hd, drop=(pa, masks["att"]))
+        if ops.use_flash(N, hd):  # the fused kernels apply the dropout mask in registers
+            if do_save:
+                a, lse = ops.attention_fwd_lse(qkv, B, N, H, hd, drop=(pa, masks["att"]))
+                P = None
+            else:
+                a, P = ops.attention_fwd(qkv, B, N, H, hd, drop=(pa, masks["att"]), need_p=False)
+        else:
+            a, P = ops.attention_fwd(qkv, B, N, H, hd, drop=(pa, masks["att"]))
     elif do_save and ops.use_flash(N, hd):
         a, lse = ops.attention_fwd_lse(qkv, B, N, H, hd)  # backward rebuilds P from the row log-sum-exp
         P = None
@@ -231,8 +238,9 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
         G["attn.proj.bias"].copy_(dx1_sum)
     ops.linear_wgrad(dt, s["a"], out=G["attn.proj.weight"])
     da = ops.linear_dgrad(dt, p["attn.proj.weight"])
-    if s.get("lse") is not None:  # flash-style: P is rebuilt inside the fused backward kernels
-        dqkv, dbqkv = ops.attention_bwd_lse(da, s["qkv"], s["a"], s["lse"], B, N, H, hd, want_colsum=True)
+    if s.get("lse") is not None:  # flash-style: P (and the dropout mask) is rebuilt inside the fused backward kernels
+        dqkv, dbqkv = ops.attention_bwd_lse(da, s["qkv"], s["a"], s["lse"], B, N, H, hd, want_colsum=True,
+                                            drop=(pa, masks["att"]) if "att" in masks else None)
     else:
         if s.get("P") is None:
             s["P"] = ops.attention_probs(s["qkv"], B, N, H, hd)

@@ -5,9 +5,9 @@ Every function launches hand-written kernels from ``_C.so``:
     (bias / GELU / dGELU / residual / pre-activation side output / bias-gradient column sums);
     forward (NT), dgrad (NN) and wgrad (TN) run on the same kernel via K-major / MN-major descriptors.
   * attention core: fused wgmma forward (keeps the row log-sum-exp) + fused backward kernels that read q/k/v in
-    place from the packed qkv buffer through 4-D TMA tensor maps; scores never reach HBM.  The un-fused path (batched
-    wgmma GEMMs + softmax / softmax-backward kernels with materialised P) remains for attention dropout and
-    B200_FUSED_ATTN_BWD=0.
+    place from the packed qkv buffer through 4-D TMA tensor maps; scores never reach HBM, attention dropout included
+    (the kernels regenerate the Philox mask of ``dropout`` in registers).  The un-fused path (batched wgmma GEMMs +
+    softmax / softmax-backward kernels with materialised P) remains for B200_FUSED_ATTN_BWD=0 and unsupported shapes.
   * LayerNorm fwd/bwd, cross-entropy, im2col, column sums, sum of squares, fused AdamW.
 
 What each group replaces in the reference (all of it reached through timm / torch_xla there):
@@ -246,13 +246,22 @@ def mean_pool_bwd(dpooled, B: int, N: int):
     return dxn
 
 
+def _drop_key(key: int) -> int:
+    return int(key) & 0x7FFFFFFFFFFFFFFF
+
+
 def attention_fwd(qkv, B: int, N: int, H: int, hd: int, drop=None, need_p: bool = True):
     """Returns (out [B*N, D], P).  P = softmax probabilities [B*H, N, ldp] for the backward, or None when
     need_p=False and the fused kernel ran (scores never reach HBM then).
-    drop = (p, key): attention dropout.  The probabilities are materialised (un-fused path), the dropped copy that
-    feeds P V comes from the Philox dropout kernel; the returned P is the un-dropped one (backward regenerates the mask)."""
+    drop = (p, key): attention dropout.  With need_p the probabilities are materialised (un-fused path), the dropped
+    copy that feeds P V comes from the Philox dropout kernel and the returned P is the un-dropped one (backward
+    regenerates the mask); without need_p the fused kernel applies the same mask in registers."""
     D = H * hd
     ldp = _pad8(N)
+    if drop is not None and not need_p and FUSED_ATTENTION and _C.attention_supported(N, hd):
+        out = torch.empty(B * N, D, dtype=qkv.dtype, device=qkv.device)
+        _C.attention_fwd(qkv, out, None, None, B, N, H, hd, float(drop[0]), _drop_key(drop[1]))
+        return out, None
     if drop is not None:
         p = attention_probs(qkv, B, N, H, hd)
         pd = dropout(p, drop[0], drop[1])
@@ -303,19 +312,28 @@ def use_flash(N: int, hd: int) -> bool:
     return FLASH_ATTENTION and flash_supported(N, hd)
 
 
-def attention_fwd_lse(qkv, B: int, N: int, H: int, hd: int):
+def attention_fwd_lse(qkv, B: int, N: int, H: int, hd: int, drop=None):
+    """drop = (p, key): attention dropout with exactly the mask ``dropout(P, p, key)`` would draw for the [B*H, N, ldp]
+    probability buffer of the un-fused path; lse stays that of the undropped scores."""
     out = torch.empty(B * N, H * hd, dtype=qkv.dtype, device=qkv.device)
     lse = torch.empty(B * H, N, dtype=torch.float32, device=qkv.device)
-    _C.attention_fwd(qkv, out, lse, None, B, N, H, hd)
+    if drop is None:
+        _C.attention_fwd(qkv, out, lse, None, B, N, H, hd)
+    else:
+        _C.attention_fwd(qkv, out, lse, None, B, N, H, hd, float(drop[0]), _drop_key(drop[1]))
     return out, lse
 
 
-def attention_bwd_lse(dout, qkv, out, lse, B: int, N: int, H: int, hd: int, want_colsum: bool = False):
+def attention_bwd_lse(dout, qkv, out, lse, B: int, N: int, H: int, hd: int, want_colsum: bool = False, drop=None):
+    """drop: the (p, key) of the forward; the kernels regenerate its mask."""
     dqkv = torch.empty(B * N, 3 * H * hd, dtype=qkv.dtype, device=qkv.device)
     delta = torch.empty(B * H, N, dtype=torch.float32, device=qkv.device)  # scratch: rowsum(dO o O)
     # the backward kernels reduce the qkv bias gradient (column sums of dq | dk | dv) from their epilogue tiles
     cs = torch.zeros(3 * H * hd, dtype=torch.float32, device=qkv.device) if want_colsum else None
-    _C.attention_bwd(qkv, dout, out, lse, delta, dqkv, cs, B, N, H, hd)
+    if drop is None:
+        _C.attention_bwd(qkv, dout, out, lse, delta, dqkv, cs, B, N, H, hd)
+    else:
+        _C.attention_bwd(qkv, dout, out, lse, delta, dqkv, cs, B, N, H, hd, float(drop[0]), _drop_key(drop[1]))
     return (dqkv, cs) if want_colsum else dqkv
 
 

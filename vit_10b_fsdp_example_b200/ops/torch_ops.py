@@ -166,24 +166,34 @@ def use_flash(N: int, hd: int) -> bool:
     return FLASH_ATTENTION
 
 
-def attention_fwd_lse(qkv, B: int, N: int, H: int, hd: int):
+def _drop_scale(p, drop):
+    """Mask times scale of attention dropout (p, key) for probabilities p [B, H, N, N]: the mask ``dropout`` draws for
+    that shape, which is the one the un-fused path applies to its P."""
+    return dropout(torch.ones_like(p, dtype=torch.float32), drop[0], drop[1])
+
+
+def attention_fwd_lse(qkv, B: int, N: int, H: int, hd: int, drop=None):
     D = H * hd
     q, k, v = _f32(qkv).view(B, N, 3, H, hd).permute(2, 0, 3, 1, 4)
     s = (q @ k.transpose(-1, -2)) * (hd ** -0.5)
-    lse = torch.logsumexp(s, dim=-1)  # [B, H, N]
-    o = (torch.exp(s - lse[..., None]) @ v).permute(0, 2, 1, 3).reshape(B * N, D).to(qkv.dtype)
+    lse = torch.logsumexp(s, dim=-1)  # [B, H, N], of the undropped scores
+    p = torch.exp(s - lse[..., None])
+    if drop is not None:
+        p = p * _drop_scale(p, drop)
+    o = (p @ v).permute(0, 2, 1, 3).reshape(B * N, D).to(qkv.dtype)
     return o, lse.reshape(B * H, N).contiguous()
 
 
-def attention_bwd_lse(dout, qkv, out, lse, B: int, N: int, H: int, hd: int, want_colsum: bool = False):
+def attention_bwd_lse(dout, qkv, out, lse, B: int, N: int, H: int, hd: int, want_colsum: bool = False, drop=None):
     D = H * hd
     q, k, v = _f32(qkv).view(B, N, 3, H, hd).permute(2, 0, 3, 1, 4)
     do = _f32(dout).view(B, N, H, hd).permute(0, 2, 1, 3)
     o = _f32(out).view(B, N, H, hd).permute(0, 2, 1, 3)
     p = torch.exp((q @ k.transpose(-1, -2)) * (hd ** -0.5) - lse.view(B, H, N, 1))
-    delta = (do * o).sum(dim=-1, keepdim=True)
-    dv = p.transpose(-1, -2) @ do
-    ds = (hd ** -0.5) * p * (do @ v.transpose(-1, -2) - delta)
+    delta = (do * o).sum(dim=-1, keepdim=True)  # = rowsum(dP o P) also with dropout: O is the dropped output
+    ms = 1.0 if drop is None else _drop_scale(p, drop)
+    dv = (p * ms).transpose(-1, -2) @ do
+    ds = (hd ** -0.5) * p * ((do @ v.transpose(-1, -2)) * ms - delta)
     dq = ds @ k
     dk = ds.transpose(-1, -2) @ q
     dqkv = torch.stack([dq, dk, dv], dim=0).permute(1, 3, 0, 2, 4).reshape(B * N, 3 * D).to(qkv.dtype)
