@@ -1,10 +1,15 @@
-"""Time the attention core with attention dropout: fused kernels with the mask drawn in registers against the un-fused
-route that materialises the probabilities, with the dropout-free fused pair as the bar.
+"""Time the attention core, fused kernels against the un-fused route that materialises the probabilities, without and
+with attention dropout (mask drawn in registers on the fused side).
 
-    python tools/bench_attention.py [--iters 20] [--warmup 3] [--p 0.1] [--out attention_bench.json]
+    python tools/bench_attention.py [--shapes vit10b,vitl] [--iters 20] [--warmup 3] [--p 0.1] [--out attention_bench.json]
 
+Shapes (SHAPES): the ViT-10B and ViT-L attention, and at 128 images of 256 tokens with 16 heads the head dims of the
+published larger ViTs: vith (ViT-H/14, hd 80), vitg (ViT-g/14, 88), vitG (ViT-G/14, 104), vite (ViT-e, 112) and sovit
+(SoViT-400m/14, 72); hd32, hd40, hd48, hd96, hd136 and hd144 cover the other fused tile widths at the same size.
 Variants, each as models/vit.py runs it for a block that keeps its activations:
   fused         attention_fwd_lse + attention_bwd_lse (no dropout)
+  unfused       attention_fwd(need_p=True), which keeps P (written by the fused forward kernel), + attention_bwd (dP
+                GEMM, softmax backward, three GEMMs); no dropout
   fused_drop    the same pair with drop=(p, key): Philox mask regenerated in the kernels, no [B*H, N, N] buffer
   unfused_drop  attention_fwd(drop=) (GEMM + softmax + dropout + GEMM) and, in the backward, attention_probs +
                 attention_bwd(drop=) (dropout of P, dP GEMM, dropout of dP, softmax backward, three GEMMs)
@@ -24,7 +29,11 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from bench_gemm import gpu_info  # noqa: E402
 
-SHAPES = {"vit10b": (128, 256, 32, 160), "vitl": (128, 196, 16, 64)}
+SHAPES = {"vit10b": (128, 256, 32, 160), "vitl": (128, 196, 16, 64), "vith": (128, 256, 16, 80),
+          "vitg": (128, 256, 16, 88), "vitG": (128, 256, 16, 104), "vite": (128, 256, 16, 112),
+          "sovit": (128, 256, 16, 72), "hd32": (128, 256, 16, 32), "hd40": (128, 256, 16, 40),
+          "hd48": (128, 256, 16, 48), "hd96": (128, 256, 16, 96), "hd136": (128, 256, 16, 136),
+          "hd144": (128, 256, 16, 144)}
 
 
 def variants(co, qkv, dout, B, N, H, hd, p):
@@ -35,6 +44,12 @@ def variants(co, qkv, dout, B, N, H, hd, p):
 
     def fused_bwd(saved):
         return co.attention_bwd_lse(dout, qkv, *saved, B, N, H, hd, want_colsum=True)
+
+    def plain_fwd():
+        return (co.attention_fwd(qkv, B, N, H, hd, need_p=True)[1],)
+
+    def plain_bwd(saved):
+        return co.attention_bwd(dout, qkv, saved[0], B, N, H, hd, want_colsum=True)
 
     def drop_fwd():
         return co.attention_fwd_lse(qkv, B, N, H, hd, drop=drop)
@@ -50,7 +65,7 @@ def variants(co, qkv, dout, B, N, H, hd, p):
         P = co.attention_probs(qkv, B, N, H, hd)
         return co.attention_bwd(dout, qkv, P, B, N, H, hd, want_colsum=True, drop=drop)
 
-    return {"fused": (fused_fwd, fused_bwd), "fused_drop": (drop_fwd, drop_bwd),
+    return {"fused": (fused_fwd, fused_bwd), "unfused": (plain_fwd, plain_bwd), "fused_drop": (drop_fwd, drop_bwd),
             "unfused_drop": (unfused_fwd, unfused_bwd)}
 
 

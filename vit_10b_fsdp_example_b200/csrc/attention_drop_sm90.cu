@@ -194,10 +194,12 @@ __global__ void __launch_bounds__(kAttnThreads) attn_fwd_drop_sm90_kernel(const 
         l0 = quad_sum(l0), l1 = quad_sum(l1);
         const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
         const int q0 = qt * kTile + r0, q1 = q0 + 8;
-        __nv_bfloat16* orow0 = p.out + (static_cast<int64_t>(b) * p.N + q0) * p.D + h * HD + cpair;
+        const int hd = head_dim<HD>(p.D, p.H);
+        __nv_bfloat16* orow0 = p.out + (static_cast<int64_t>(b) * p.N + q0) * p.D + h * hd + cpair;
         __nv_bfloat16* orow1 = orow0 + 8 * static_cast<int64_t>(p.D);
 #pragma unroll
         for (int j = 0; j < HD / 8; ++j) {
+            if (j * 8 >= hd) continue;  // zero-padded columns of the tile
             if (q0 < p.N) *reinterpret_cast<uint32_t*>(orow0 + j * 8) = pack_bf16x2(o[4 * j] * inv0, o[4 * j + 1] * inv0);
             if (q1 < p.N) *reinterpret_cast<uint32_t*>(orow1 + j * 8) = pack_bf16x2(o[4 * j + 2] * inv1, o[4 * j + 3] * inv1);
         }
@@ -351,11 +353,12 @@ __global__ void __launch_bounds__(kAttnThreads) attn_bwd_drop_sm90_kernel(const 
             __syncthreads();  // every warp is done with slot s (and, after the last tile, with the owned tiles)
         }
 
+        const int hd = head_dim<HD>(p.D, p.H);
         if constexpr (kRole == 0) {
-            store_grad_tile<HD>(acc2, p, b, ot * kTile, r0, cpair, p.D + h * HD, lane);
-            store_grad_tile<HD>(acc1, p, b, ot * kTile, r0, cpair, 2 * p.D + h * HD, lane);
+            store_grad_tile<HD>(acc2, p, b, ot * kTile, r0, cpair, p.D + h * hd, lane);
+            store_grad_tile<HD>(acc1, p, b, ot * kTile, r0, cpair, 2 * p.D + h * hd, lane);
         } else {
-            store_grad_tile<HD>(acc1, p, b, ot * kTile, r0, cpair, h * HD, lane);
+            store_grad_tile<HD>(acc1, p, b, ot * kTile, r0, cpair, h * hd, lane);
         }
     }
 }
@@ -377,9 +380,10 @@ void launch_fwd_drop(const __nv_bfloat16* qkv, int64_t ld_qkv, const AttnParams&
     static bool attr_set = false;
     if (!attr_set) set_smem(kern, kSmem), attr_set = true;
     GemmOperand ops[3];
-    qkv_operands(qkv, ld_qkv, p.N, p.H, HD, ops);
-    const CUtensorMap tq = tile_map<HD>(ops[0], p.B, p.N), tk = tile_map<HD>(ops[1], p.B, p.N),
-                      tv = tile_map<HD>(ops[2], p.B, p.N);
+    const int hd = p.D / p.H;
+    qkv_operands(qkv, ld_qkv, p.N, p.H, hd, ops);
+    const CUtensorMap tq = tile_map<HD>(ops[0], p.B, p.N, hd), tk = tile_map<HD>(ops[1], p.B, p.N, hd),
+                      tv = tile_map<HD>(ops[2], p.B, p.N, hd);
     const int items = (p.N + kTile - 1) / kTile * p.H * p.B;
     kern<<<items, kAttnThreads, kSmem, stream>>>(tq, tk, tv, p, d);
     check_launch("attention forward (dropout) launch");
@@ -394,10 +398,11 @@ void launch_bwd_drop(const __nv_bfloat16* qkv, int64_t ld_qkv, const __nv_bfloat
     static bool attr_set = false;
     if (!attr_set) set_smem(kern_kv, kSmem), set_smem(kern_q, kSmem), attr_set = true;
     GemmOperand ops[3], od;
-    qkv_operands(qkv, ld_qkv, p.N, p.H, HD, ops);
-    od.ptr = dout, od.ld = ld_do, od.nb_inner = p.H, od.stride_b_inner = HD;
-    const CUtensorMap tq = tile_map<HD>(ops[0], p.B, p.N), tk = tile_map<HD>(ops[1], p.B, p.N),
-                      tv = tile_map<HD>(ops[2], p.B, p.N), tdo = tile_map<HD>(od, p.B, p.N);
+    const int hd = p.D / p.H;
+    qkv_operands(qkv, ld_qkv, p.N, p.H, hd, ops);
+    od.ptr = dout, od.ld = ld_do, od.nb_inner = p.H, od.stride_b_inner = hd;
+    const CUtensorMap tq = tile_map<HD>(ops[0], p.B, p.N, hd), tk = tile_map<HD>(ops[1], p.B, p.N, hd),
+                      tv = tile_map<HD>(ops[2], p.B, p.N, hd), tdo = tile_map<HD>(od, p.B, p.N, hd);
     const int items = (p.N + kTile - 1) / kTile * p.H * p.B;
     kern_kv<<<items, kAttnThreads, kSmem, stream>>>(tq, tk, tv, tdo, p, d);
     check_launch("attention backward (dK/dV, dropout) launch");
@@ -416,9 +421,8 @@ void attention_fwd_drop(const __nv_bfloat16* qkv, int64_t ld_qkv, __nv_bfloat16*
     p.scale = 1.0f / sqrtf(static_cast<float>(hd));
     p.scale_log2 = p.scale * kLog2e;
     p.out = out, p.lse = lse, p.p = nullptr, p.ldp = 0;
-    if (hd == 64) launch_fwd_drop<64>(qkv, ld_qkv, p, d, stream);
-    else if (hd == 128) launch_fwd_drop<128>(qkv, ld_qkv, p, d, stream);
-    else launch_fwd_drop<160>(qkv, ld_qkv, p, d, stream);
+    dispatch_tile_width(hd, "attention_fwd",
+                        [&](auto w) { launch_fwd_drop<decltype(w)::value>(qkv, ld_qkv, p, d, stream); });
 }
 
 void attention_bwd_drop(const __nv_bfloat16* qkv, int64_t ld_qkv, const __nv_bfloat16* dout, int64_t ld_do,
@@ -431,9 +435,8 @@ void attention_bwd_drop(const __nv_bfloat16* qkv, int64_t ld_qkv, const __nv_bfl
     p.scale = 1.0f / sqrtf(static_cast<float>(hd));
     p.scale_log2 = p.scale * kLog2e;
     p.lse = lse, p.delta = delta, p.dqkv = dqkv, p.colsum = colsum;
-    if (hd == 64) launch_bwd_drop<64>(qkv, ld_qkv, dout, ld_do, p, d, stream);
-    else if (hd == 128) launch_bwd_drop<128>(qkv, ld_qkv, dout, ld_do, p, d, stream);
-    else launch_bwd_drop<160>(qkv, ld_qkv, dout, ld_do, p, d, stream);
+    dispatch_tile_width(hd, "attention_bwd",
+                        [&](auto w) { launch_bwd_drop<decltype(w)::value>(qkv, ld_qkv, dout, ld_do, p, d, stream); });
 }
 
 }  // namespace b200

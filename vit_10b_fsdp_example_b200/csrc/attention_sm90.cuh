@@ -8,6 +8,7 @@
 #include <cstdint>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 #include "gemm_sm90.h"
 #include "ptx.cuh"
@@ -21,17 +22,25 @@ constexpr int kAttnThreads = 128;  // one warpgroup
 constexpr int kTile = 64;          // rows of every Q / K / V / dO tile
 constexpr float kLog2e = 1.4426950408889634f;
 
-// hd-contiguous tiles use the widest swizzle atom that divides hd: 64 elements (SWIZZLE_128B) or 32 (SWIZZLE_64B).
+// hd-contiguous tiles use the widest swizzle atom that divides the tile width HD: 64 elements (SWIZZLE_128B), 32
+// (SWIZZLE_64B) or 16 (SWIZZLE_32B).
 template <int HD>
 struct TileCfg {
-    static constexpr int W = (HD % 64 == 0) ? 64 : 32;
+    static constexpr int W = (HD % 64 == 0) ? 64 : (HD % 32 == 0) ? 32 : 16;
     static constexpr int kAtoms = HD / W;
     static constexpr int kRowBytes = W * 2;
-    static constexpr uint32_t kMode = (W == 64) ? 1u : 2u;  // wgmma descriptor swizzle mode
+    static constexpr uint32_t kMode = (W == 64) ? 1u : (W == 32) ? 2u : 3u;  // wgmma descriptor swizzle mode
     static constexpr int kAtomBytes = kTile * kRowBytes;
     static constexpr int kTileBytes = kTile * HD * 2;
-    static_assert(HD % 32 == 0 && HD <= 256, "unsupported head dim");
+    // Widths 64 / 128 / 160 are compiled for hd == HD.  The others read hd (HD - 16 < hd <= HD) at run time; TMA
+    // zero-fills tile columns hd..HD-1, which add nothing to S or dP, and the epilogues store columns < hd only.
+    static constexpr bool kFixedHd = HD == 64 || HD == 128 || HD == 160;
+    static_assert(HD % 16 == 0 && HD <= 256, "unsupported tile width");
 };
+
+// Head dim served by the kernels of tile width HD.
+template <int HD>
+__device__ __forceinline__ int head_dim(int D, int H) { return TileCfg<HD>::kFixedHd ? HD : D / H; }
 
 // One box per swizzle atom (W hd-columns x 64 rows); rows past the end of the image are zero-filled.
 template <int HD>
@@ -105,16 +114,18 @@ struct BwdParams {
     float* colsum;        // [3*D] or null
 };
 
-// acc (64 x hd, rows = tokens of this tile) -> dqkv[token, col0 + :] and, optionally, its column sums.
+// acc (64 x HD, rows = tokens of this tile) -> dqkv[token, col0 + :hd] and, optionally, its column sums.
 template <int HD>
 __device__ __forceinline__ void store_grad_tile(const float (&acc)[HD / 2], const BwdParams& p, int b, int row0, int r0,
                                                 int cpair, int col0, uint32_t lane) {
+    const int hd = head_dim<HD>(p.D, p.H);
     const int t0 = row0 + r0, t1 = t0 + 8;
     const bool ok0 = t0 < p.N, ok1 = t1 < p.N;
     __nv_bfloat16* g0 = p.dqkv + (static_cast<int64_t>(b) * p.N + t0) * (3 * p.D) + col0 + cpair;
     __nv_bfloat16* g1 = g0 + 8 * static_cast<int64_t>(3 * p.D);
 #pragma unroll
     for (int j = 0; j < HD / 8; ++j) {
+        if (j * 8 >= hd) continue;  // hd % 8 == 0: an 8-column group lies wholly inside or past the head
         const uint32_t w0 = ok0 ? pack_bf16x2(acc[4 * j], acc[4 * j + 1]) : 0u;
         const uint32_t w1 = ok1 ? pack_bf16x2(acc[4 * j + 2], acc[4 * j + 3]) : 0u;
         if (ok0) *reinterpret_cast<uint32_t*>(g0 + j * 8) = w0;
@@ -155,14 +166,41 @@ void qkv_operands(const __nv_bfloat16* qkv, int64_t ld_qkv, int N, int H, int hd
     }
 }
 
-// Tensor map of one 64-row tile shape over a [B, N, H, hd] view (rows past N of an image read as zeros).
+// Tensor map of one 64-row tile shape over a [B, N, H, hd] view (rows past N of an image and columns past hd of a
+// head read as zeros).
 template <int HD>
-CUtensorMap tile_map(GemmOperand op, int B, int N) {
+CUtensorMap tile_map(GemmOperand op, int B, int N, int hd) {
     op.nb_outer = B, op.stride_b_outer = static_cast<int64_t>(N) * op.ld;
-    return make_tensor_map_4d(op, HD, N, TileCfg<HD>::W, kTile, TileCfg<HD>::kRowBytes);
+    return make_tensor_map_4d(op, hd, N, TileCfg<HD>::W, kTile, TileCfg<HD>::kRowBytes);
 }
 
-bool shape_ok(int N, int hd) { return N > 0 && N % 2 == 0 && (hd == 64 || hd == 128 || hd == 160); }
+// Tile width the kernels run head dim hd at (hd rounded up to 16), or 0 when they do not take hd.  hd % 8 == 0 because
+// TMA needs the head stride (hd * 2 bytes) to be a multiple of 16.  hd = 56 / 120 / 152 would need zero-padded
+// kernels at the widths 64 / 128 / 160, which are compiled for hd == width only.
+constexpr int tile_width(int hd) {
+    if (hd % 8 != 0 || hd < 32 || hd > 160) return 0;
+    const int w = (hd + 15) / 16 * 16;
+    return (w == 64 || w == 128 || w == 160) && w != hd ? 0 : w;
+}
+
+bool shape_ok(int N, int hd) { return N > 0 && N % 2 == 0 && tile_width(hd) != 0; }
+
+// Calls f(std::integral_constant<int, W>) with the tile width W of hd; throws when no kernel takes hd.
+template <typename F>
+void dispatch_tile_width(int hd, const char* what, F&& f) {
+    switch (tile_width(hd)) {
+        case 32: return f(std::integral_constant<int, 32>());
+        case 48: return f(std::integral_constant<int, 48>());
+        case 64: return f(std::integral_constant<int, 64>());
+        case 80: return f(std::integral_constant<int, 80>());
+        case 96: return f(std::integral_constant<int, 96>());
+        case 112: return f(std::integral_constant<int, 112>());
+        case 128: return f(std::integral_constant<int, 128>());
+        case 144: return f(std::integral_constant<int, 144>());
+        case 160: return f(std::integral_constant<int, 160>());
+    }
+    throw std::runtime_error(std::string(what) + ": no kernel for head dim " + std::to_string(hd));
+}
 
 }  // namespace
 

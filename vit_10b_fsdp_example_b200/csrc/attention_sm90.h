@@ -6,7 +6,9 @@
 
 namespace b200 {
 
-// Even N, head dim 64 / 128 / 160.
+// Whether the model routes (N, hd) through the fused kernels: even N and head dim 32, 40, 48, 64, 128 or 160.  The
+// kernels themselves also take hd 72, 80, 88, 96, 104, 112, 136 and 144 (attention_sm90.cu says why those are not
+// routed); attention_fwd / attention_bwd throw on any other head dim.
 bool attention_supported(int N, int hd);
 
 // qkv: packed [B*N, 3*H*hd] (row stride ld_qkv).  out: [B*N, H*hd].  lse: [B*H, N] fp32 or null.
