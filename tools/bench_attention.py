@@ -6,6 +6,9 @@ with attention dropout (mask drawn in registers on the fused side).
 Shapes (SHAPES): the ViT-10B and ViT-L attention, and at 128 images of 256 tokens with 16 heads the head dims of the
 published larger ViTs: vith (ViT-H/14, hd 80), vitg (ViT-g/14, 88), vitG (ViT-G/14, 104), vite (ViT-e, 112) and sovit
 (SoViT-400m/14, 72); hd32, hd40, hd48, hd96, hd136 and hd144 cover the other fused tile widths at the same size.
+Token counts the model runs un-fused: b32 (ViT-B/32 at 224 px, N 49), vit10b_518 (ViT-10B at 518 px, N 1369), vitG_518
+(ViT-G/14 at 518 px, N 1369, hd 104), vith_476 (ViT-H/14 at 476 px, N 1156, hd 80) and vite_588 (ViT-e at 588 px, N 1764,
+hd 112); at odd N only the un-fused variants run.
 Variants, each as models/vit.py runs it for a block that keeps its activations:
   fused         attention_fwd_lse + attention_bwd_lse (no dropout)
   unfused       attention_fwd(need_p=True), which keeps P (written by the fused forward kernel), + attention_bwd (dP
@@ -33,7 +36,11 @@ SHAPES = {"vit10b": (128, 256, 32, 160), "vitl": (128, 196, 16, 64), "vith": (12
           "vitg": (128, 256, 16, 88), "vitG": (128, 256, 16, 104), "vite": (128, 256, 16, 112),
           "sovit": (128, 256, 16, 72), "hd32": (128, 256, 16, 32), "hd40": (128, 256, 16, 40),
           "hd48": (128, 256, 16, 48), "hd96": (128, 256, 16, 96), "hd136": (128, 256, 16, 136),
-          "hd144": (128, 256, 16, 144)}
+          "hd144": (128, 256, 16, 144),
+          # grids the fused pair is not routed for: odd N, and N > 1024 at head dims that are not routed.  Batches are
+          # sized so that the un-fused variants, which keep P [B*H, N, pad8(N)], fit 80 GB.
+          "b32": (1024, 49, 12, 64), "vit10b_518": (32, 1369, 32, 160), "vitG_518": (32, 1369, 16, 104),
+          "vith_476": (32, 1156, 16, 80), "vite_588": (32, 1764, 16, 112)}
 
 
 def variants(co, qkv, dout, B, N, H, hd, p):
@@ -65,8 +72,11 @@ def variants(co, qkv, dout, B, N, H, hd, p):
         P = co.attention_probs(qkv, B, N, H, hd)
         return co.attention_bwd(dout, qkv, P, B, N, H, hd, want_colsum=True, drop=drop)
 
-    return {"fused": (fused_fwd, fused_bwd), "unfused": (plain_fwd, plain_bwd), "fused_drop": (drop_fwd, drop_bwd),
-            "unfused_drop": (unfused_fwd, unfused_bwd)}
+    vs = {"fused": (fused_fwd, fused_bwd), "unfused": (plain_fwd, plain_bwd), "fused_drop": (drop_fwd, drop_bwd),
+          "unfused_drop": (unfused_fwd, unfused_bwd)}
+    if N % 2:  # the fused kernels take even N only
+        del vs["fused"], vs["fused_drop"]
+    return vs
 
 
 def peak_bytes(fwd, bwd):

@@ -631,6 +631,193 @@ __global__ void softmax_bwd_kernel(__nv_bfloat16* __restrict__ dp, const __nv_bf
 }
 
 // ------------------------------------------------------------------------------------------------
+// Row softmax fwd / bwd for the rows the pair kernels above do not take: odd n (an odd patch grid, e.g. 7 x 7 or
+// 37 x 37 tokens) and n > 1024.  Same math (fp32, exp2 with the scale folded in), one warp per row, 16-byte vectors:
+// ld must be a multiple of 8.  The last vector of a row may be partial; its columns n..ld-1 are padding, masked on
+// load and never written.  Up to n = 2048 the row stays in registers (kVecs vectors per lane); longer rows stream
+// twice through L1/L2: online max / sum (fwd) or the dot product (bwd), then the write.
+// ------------------------------------------------------------------------------------------------
+constexpr int kSoftmaxRegMaxN = 32 * 8 * 8;
+
+// Scores of vector `idx` of a row, times sl2; columns >= n become -inf.
+__device__ __forceinline__ void load_scores8(const __nv_bfloat16* r, int idx, int n, float sl2, float (&f)[8]) {
+    unpack8(reinterpret_cast<const uint4*>(r)[idx], f);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) f[q] = idx * 8 + q < n ? f[q] * sl2 : -INFINITY;
+}
+
+// Vector `idx` of a row; columns >= n read as 0.
+__device__ __forceinline__ void load_masked8(const __nv_bfloat16* r, int idx, int n, float (&f)[8]) {
+    unpack8(reinterpret_cast<const uint4*>(r)[idx], f);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) f[q] = idx * 8 + q < n ? f[q] : 0.f;
+}
+
+// Writes the columns < n of vector `idx`: one 16-byte store, or element stores for the partial last vector.
+__device__ __forceinline__ void store_row8(__nv_bfloat16* r, int idx, int n, const float (&f)[8]) {
+    if (idx * 8 + 8 <= n) {
+        reinterpret_cast<uint4*>(r)[idx] = pack8(f);
+    } else {
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+            if (idx * 8 + q < n) r[idx * 8 + q] = __float2bfloat16_rn(f[q]);
+    }
+}
+
+template <int kVecs>  // 16-byte vectors per lane
+__global__ void __launch_bounds__(256) softmax_fwd_vec_kernel(__nv_bfloat16* __restrict__ s, int64_t rows, int n,
+                                                              int64_t ld, float scale) {
+    const int64_t row = static_cast<int64_t>(blockIdx.x) * (blockDim.x / 32) + threadIdx.x / 32;
+    if (row >= rows) return;
+    const int lane = threadIdx.x % 32;
+    __nv_bfloat16* r = s + row * ld;
+    const int nvec = (n + 7) / 8;
+    const float sl2 = scale * 1.4426950408889634f;
+    float v[kVecs][8];
+    float mx = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < kVecs; ++i) {
+        const int idx = lane + i * 32;
+        if (idx < nvec) {
+            load_scores8(r, idx, n, sl2, v[i]);
+        } else {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) v[i][q] = -INFINITY;
+        }
+#pragma unroll
+        for (int q = 0; q < 8; ++q) mx = fmaxf(mx, v[i][q]);
+    }
+    mx = warp_max(mx);
+    float sum = 0.f;
+#pragma unroll
+    for (int i = 0; i < kVecs; ++i) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+            v[i][q] = exp2f(v[i][q] - mx);
+            sum += v[i][q];
+        }
+    }
+    sum = warp_sum(sum);
+    const float inv = 1.0f / sum;
+#pragma unroll
+    for (int i = 0; i < kVecs; ++i) {
+        const int idx = lane + i * 32;
+        if (idx < nvec) {
+#pragma unroll
+            for (int q = 0; q < 8; ++q) v[i][q] *= inv;
+            store_row8(r, idx, n, v[i]);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) softmax_fwd_long_kernel(__nv_bfloat16* __restrict__ s, int64_t rows, int n,
+                                                               int64_t ld, float scale) {
+    const int64_t row = static_cast<int64_t>(blockIdx.x) * (blockDim.x / 32) + threadIdx.x / 32;
+    if (row >= rows) return;
+    const int lane = threadIdx.x % 32;
+    __nv_bfloat16* r = s + row * ld;
+    const int nvec = (n + 7) / 8;
+    const float sl2 = scale * 1.4426950408889634f;
+    // pass 1: this lane's running max and sum of exp2(x - max), rescaled whenever the max grows
+    float mx = -INFINITY, sum = 0.f;
+    for (int idx = lane; idx < nvec; idx += 32) {
+        float f[8];
+        load_scores8(r, idx, n, sl2, f);
+        float vm = f[0];
+#pragma unroll
+        for (int q = 1; q < 8; ++q) vm = fmaxf(vm, f[q]);
+        if (vm > mx) {
+            sum *= exp2f(mx - vm);
+            mx = vm;
+        }
+#pragma unroll
+        for (int q = 0; q < 8; ++q) sum += exp2f(f[q] - mx);
+    }
+    const float row_max = warp_max(mx);
+    sum = warp_sum(mx == -INFINITY ? 0.f : sum * exp2f(mx - row_max));
+    const float inv = 1.0f / sum;
+    // pass 2: normalised write
+    for (int idx = lane; idx < nvec; idx += 32) {
+        float f[8];
+        load_scores8(r, idx, n, sl2, f);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) f[q] = exp2f(f[q] - row_max) * inv;
+        store_row8(r, idx, n, f);
+    }
+}
+
+// dS = scale * P * (dP - sum_j dP_j P_j), in place on dP; P and dP stay packed in registers.
+template <int kVecs>
+__global__ void __launch_bounds__(256) softmax_bwd_vec_kernel(__nv_bfloat16* __restrict__ dp,
+                                                              const __nv_bfloat16* __restrict__ p, int64_t rows, int n,
+                                                              int64_t ld, float scale) {
+    const int64_t row = static_cast<int64_t>(blockIdx.x) * (blockDim.x / 32) + threadIdx.x / 32;
+    if (row >= rows) return;
+    const int lane = threadIdx.x % 32;
+    __nv_bfloat16* dr = dp + row * ld;
+    const __nv_bfloat16* pr = p + row * ld;
+    const int nvec = (n + 7) / 8;
+    uint4 pw[kVecs], dw[kVecs];
+    float dot = 0.f;
+#pragma unroll
+    for (int i = 0; i < kVecs; ++i) {
+        const int idx = lane + i * 32;
+        pw[i] = dw[i] = make_uint4(0, 0, 0, 0);
+        if (idx < nvec) {
+            pw[i] = reinterpret_cast<const uint4*>(pr)[idx];
+            dw[i] = reinterpret_cast<const uint4*>(dr)[idx];
+            float pf[8], df[8];
+            unpack8(pw[i], pf);
+            unpack8(dw[i], df);
+#pragma unroll
+            for (int q = 0; q < 8; ++q)
+                if (idx * 8 + q < n) dot += pf[q] * df[q];
+        }
+    }
+    dot = warp_sum(dot);
+#pragma unroll
+    for (int i = 0; i < kVecs; ++i) {
+        const int idx = lane + i * 32;
+        if (idx < nvec) {
+            float pf[8], df[8];
+            unpack8(pw[i], pf);
+            unpack8(dw[i], df);
+#pragma unroll
+            for (int q = 0; q < 8; ++q) df[q] = scale * pf[q] * (df[q] - dot);
+            store_row8(dr, idx, n, df);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) softmax_bwd_long_kernel(__nv_bfloat16* __restrict__ dp,
+                                                               const __nv_bfloat16* __restrict__ p, int64_t rows,
+                                                               int n, int64_t ld, float scale) {
+    const int64_t row = static_cast<int64_t>(blockIdx.x) * (blockDim.x / 32) + threadIdx.x / 32;
+    if (row >= rows) return;
+    const int lane = threadIdx.x % 32;
+    __nv_bfloat16* dr = dp + row * ld;
+    const __nv_bfloat16* pr = p + row * ld;
+    const int nvec = (n + 7) / 8;
+    float dot = 0.f;
+    for (int idx = lane; idx < nvec; idx += 32) {
+        float pf[8], df[8];
+        load_masked8(pr, idx, n, pf);
+        load_masked8(dr, idx, n, df);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) dot += pf[q] * df[q];
+    }
+    dot = warp_sum(dot);
+    for (int idx = lane; idx < nvec; idx += 32) {
+        float pf[8], df[8];
+        load_masked8(pr, idx, n, pf);
+        load_masked8(dr, idx, n, df);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) df[q] = scale * pf[q] * (df[q] - dot);
+        store_row8(dr, idx, n, df);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Cross entropy: loss += mean_b( logsumexp(logits_b) - logits_b[target_b] ), dlogits = (softmax - 1hot)/B
 // One CTA per row.
 // ------------------------------------------------------------------------------------------------
@@ -973,23 +1160,56 @@ void layernorm_bwd(const __nv_bfloat16* dy, const __nv_bfloat16* x, const __nv_b
     if (pairs_per_lane <= 2) KERNEL<2><<<grid, 256, 0, stream>>>(__VA_ARGS__);                     \
     else if (pairs_per_lane <= 4) KERNEL<4><<<grid, 256, 0, stream>>>(__VA_ARGS__);                \
     else if (pairs_per_lane <= 9) KERNEL<9><<<grid, 256, 0, stream>>>(__VA_ARGS__);                \
-    else if (pairs_per_lane <= 16) KERNEL<16><<<grid, 256, 0, stream>>>(__VA_ARGS__);              \
-    else throw std::runtime_error("softmax: row length > 1024 not supported");
+    else KERNEL<16><<<grid, 256, 0, stream>>>(__VA_ARGS__);
+
+// The bf16x2 pair kernels take even n <= 1024; the vector kernels take every other row length.
+static bool softmax_pairs(int n) { return n % 2 == 0 && n <= 1024; }
+
+static void check_softmax_args(const void* a, const void* b, int n, int64_t ld) {
+    if (n < 1) throw std::runtime_error("softmax: row length n must be >= 1");
+    if (ld < n) throw std::runtime_error("softmax: ld must be >= row length n");
+    if (softmax_pairs(n)) {
+        if (ld % 2 != 0) throw std::runtime_error("softmax: ld must be even");
+    } else {
+        if (ld % 8 != 0) throw std::runtime_error("softmax: ld must be a multiple of 8 for odd n or n > 1024");
+        if ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) % 16 != 0)
+            throw std::runtime_error("softmax: buffers must be 16-byte aligned for odd n or n > 1024");
+    }
+}
+
+#define SM_VEC_DISPATCH(KERNEL, LONG_KERNEL, ...)                                                  \
+    if (vecs_per_lane <= 1) KERNEL<1><<<grid, 256, 0, stream>>>(__VA_ARGS__);                      \
+    else if (vecs_per_lane <= 2) KERNEL<2><<<grid, 256, 0, stream>>>(__VA_ARGS__);                 \
+    else if (vecs_per_lane <= 4) KERNEL<4><<<grid, 256, 0, stream>>>(__VA_ARGS__);                 \
+    else if (n <= kSoftmaxRegMaxN) KERNEL<8><<<grid, 256, 0, stream>>>(__VA_ARGS__);               \
+    else LONG_KERNEL<<<grid, 256, 0, stream>>>(__VA_ARGS__);
 
 void softmax_fwd(__nv_bfloat16* s, int64_t rows, int n, int64_t ld, float scale, cudaStream_t stream) {
-    if (n % 2 != 0 || ld % 2 != 0) throw std::runtime_error("softmax: row length and ld must be even");
-    const int pairs_per_lane = (n / 2 + 31) / 32;
+    check_softmax_args(s, s, n, ld);
     const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
-    SM_DISPATCH(softmax_fwd_kernel, s, rows, n, ld, scale);
+    if (softmax_pairs(n)) {
+        const int pairs_per_lane = (n / 2 + 31) / 32;
+        SM_DISPATCH(softmax_fwd_kernel, s, rows, n, ld, scale);
+    } else {
+        if (rows == 0) return;
+        const int vecs_per_lane = ((n + 7) / 8 + 31) / 32;
+        SM_VEC_DISPATCH(softmax_fwd_vec_kernel, softmax_fwd_long_kernel, s, rows, n, ld, scale);
+    }
     check_launch("softmax_fwd");
 }
 
 void softmax_bwd(__nv_bfloat16* dp, const __nv_bfloat16* p, int64_t rows, int n, int64_t ld, float scale,
                  cudaStream_t stream) {
-    if (n % 2 != 0 || ld % 2 != 0) throw std::runtime_error("softmax: row length and ld must be even");
-    const int pairs_per_lane = (n / 2 + 31) / 32;
+    check_softmax_args(dp, p, n, ld);
     const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
-    SM_DISPATCH(softmax_bwd_kernel, dp, p, rows, n, ld, scale);
+    if (softmax_pairs(n)) {
+        const int pairs_per_lane = (n / 2 + 31) / 32;
+        SM_DISPATCH(softmax_bwd_kernel, dp, p, rows, n, ld, scale);
+    } else {
+        if (rows == 0) return;
+        const int vecs_per_lane = ((n + 7) / 8 + 31) / 32;
+        SM_VEC_DISPATCH(softmax_bwd_vec_kernel, softmax_bwd_long_kernel, dp, p, rows, n, ld, scale);
+    }
     check_launch("softmax_bwd");
 }
 

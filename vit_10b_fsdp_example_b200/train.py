@@ -28,7 +28,7 @@ from .data import build_datasets
 from .launch import Runtime
 from .parallel import FSDPViT, GraphedTrainStep, ShardedAdamW
 from .utils import SmoothedValue, get_warmup_cosine_scheduler
-from .utils.checkpoint import load_ckpt, normalize_full_state_dict_keys, save_ckpt
+from .utils.checkpoint import load_ckpt, normalize_full_state_dict_keys, resize_pos_embed, save_ckpt
 
 
 def resolve_dtype(cfg, device: torch.device) -> torch.dtype:
@@ -196,7 +196,14 @@ class Trainer:
 
         if getattr(cfg, "init_from_full_ckpt", ""):
             full = torch.load(cfg.init_from_full_ckpt, map_location="cpu", weights_only=False)
-            self.model.load_full_state_dict(normalize_full_state_dict_keys(full.get("model", full)))
+            state = normalize_full_state_dict_keys(full.get("model", full))
+            mcfg = self.model.cfg
+            if "pos_embed" in state:
+                pos = state["pos_embed"]
+                state["pos_embed"] = resize_pos_embed(pos, mcfg.num_patches, mcfg.embed_dim)
+                if state["pos_embed"] is not pos:
+                    say(f"pos_embed resampled from {pos.shape[1]} to {mcfg.num_patches} tokens (bicubic)")
+            self.model.load_full_state_dict(state)
             say(f"parameters initialised from the consolidated checkpoint {cfg.init_from_full_ckpt}")
             del full
         os.makedirs(cfg.ckpt_dir, exist_ok=True)
