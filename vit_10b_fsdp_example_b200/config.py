@@ -68,7 +68,17 @@ def build_arg_parser() -> argparse.ArgumentParser:
     parser.add_argument("--h2d_prefetch", type=int, default=2, help="batches staged ahead on the copy stream")
     parser.add_argument("--cuda_graph", action="store_true",
                         help="capture the whole training step (fwd, bwd, collectives, clip, AdamW) in one CUDA graph")
+    parser.add_argument("--drop_path_rate", type=_drop_path_rate, default=0.0,
+                        help="stochastic depth (timm drop_path): block i drops each residual branch per sample with "
+                             "rate linspace(0, drop_path_rate, num_blocks)[i]; 0 = off")
     return parser
+
+
+def _drop_path_rate(s: str) -> float:
+    v = float(s)
+    if not 0.0 <= v < 1.0:
+        raise argparse.ArgumentTypeError(f"--drop_path_rate must be in [0, 1), got {s}")
+    return v
 
 
 def parse_args(argv=None) -> argparse.Namespace:
@@ -87,13 +97,18 @@ class ViTConfig:
     att_dropout: float = 0.0
     mlp_dropout: float = 0.0
     num_classes: int = 1000
+    drop_path_rate: float = 0.0  # stochastic depth; block i uses linspace(0, drop_path_rate, num_blocks)[i]
+
+    def __post_init__(self):
+        if not 0.0 <= self.drop_path_rate < 1.0:
+            raise ValueError(f"drop_path_rate must be in [0, 1), got {self.drop_path_rate}")
 
     @classmethod
     def from_args(cls, cfg) -> "ViTConfig":
         return cls(image_size=cfg.image_size, patch_size=cfg.patch_size, embed_dim=cfg.embed_dim,
                    num_heads=cfg.num_heads, num_blocks=cfg.num_blocks, mlp_ratio=cfg.mlp_ratio,
                    pos_dropout=cfg.pos_dropout, att_dropout=cfg.att_dropout, mlp_dropout=cfg.mlp_dropout,
-                   num_classes=cfg.num_classes)
+                   num_classes=cfg.num_classes, drop_path_rate=getattr(cfg, "drop_path_rate", 0.0))
 
     @property
     def grid(self) -> int:

@@ -34,7 +34,8 @@ inline cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().strea
 void gemm(Tensor a, int64_t lda, int64_t major_a, Tensor b, int64_t ldb, int64_t major_b, Tensor d, int64_t ldd,
           int64_t M, int64_t N, int64_t K, OptT bias, OptT residual, int64_t ld_res, int64_t res_row_mod, OptT aux_in,
           int64_t ld_aux, OptT aux_out, int64_t ld_aux_out, OptT colsum, int64_t colsum_bi_stride, int64_t act,
-          std::vector<int64_t> batch, int64_t block_n, int64_t cluster, int64_t max_ctas, std::vector<int64_t> ag) {
+          std::vector<int64_t> batch, int64_t block_n, int64_t cluster, int64_t max_ctas, std::vector<int64_t> ag,
+          OptT row_scale, int64_t rows_per_scale) {
     c10::cuda::CUDAGuard guard(a.device());
     b200::GemmOperand A, B, D, X;
     A.ptr = bf16_ptr(a), A.ld = lda;
@@ -54,6 +55,11 @@ void gemm(Tensor a, int64_t lda, int64_t major_a, Tensor b, int64_t ldb, int64_t
     if (aux_in.has_value()) e.aux_in = bf16_ptr(*aux_in), e.ld_aux = ld_aux;
     if (colsum.has_value()) e.colsum = f32_ptr(*colsum), e.colsum_bi_stride = colsum_bi_stride;
     e.act = static_cast<int>(act);
+    if (row_scale.has_value()) {
+        TORCH_CHECK(row_scale->is_contiguous() && row_scale->numel() * rows_per_scale >= M,
+                    "gemm: row_scale must be contiguous with one entry per rows_per_scale rows");
+        e.row_scale = f32_ptr(*row_scale), e.rows_per_scale = (int)rows_per_scale;
+    }
     if (aux_out.has_value()) {
         X = D;
         X.ptr = bf16_ptr(*aux_out), X.ld = ld_aux_out;
@@ -153,6 +159,20 @@ void dropout(Tensor x, Tensor y, double p, int64_t key) {
     c10::cuda::CUDAGuard guard(x.device());
     TORCH_CHECK(x.is_contiguous() && y.is_contiguous() && x.numel() == y.numel(), "dropout: contiguous, same size");
     b200::dropout(bf16_ptr(x), bf16_mut(y), x.numel(), (float)p, (uint64_t)key, cur_stream());
+}
+void drop_path_scale(Tensor scale, int64_t sample_offset, double p, int64_t key) {
+    c10::cuda::CUDAGuard guard(scale.device());
+    TORCH_CHECK(scale.is_contiguous() && scale.dim() == 1, "drop_path_scale: contiguous [B] fp32 output");
+    b200::drop_path_scale(f32_ptr(scale), (int)scale.numel(), sample_offset, (float)p, (uint64_t)key, cur_stream());
+}
+void drop_path_bwd(Tensor dy, Tensor scale, Tensor dt, Tensor colsum, int64_t N) {
+    c10::cuda::CUDAGuard guard(dy.device());
+    TORCH_CHECK(dy.dim() == 2 && dy.is_contiguous() && dt.is_contiguous() && dt.sizes() == dy.sizes(),
+                "drop_path_bwd: contiguous [T, C] dy and dt");
+    TORCH_CHECK(scale.is_contiguous() && scale.numel() * N == dy.size(0), "drop_path_bwd: one scale per N rows");
+    TORCH_CHECK(colsum.is_contiguous() && colsum.numel() == dy.size(1), "drop_path_bwd: colsum must be [C]");
+    b200::drop_path_bwd(bf16_ptr(dy), f32_ptr(scale), bf16_mut(dt), f32_ptr(colsum), dy.size(0), (int)dy.size(1),
+                        (int)N, cur_stream());
 }
 void meanpool_fwd(Tensor xn, Tensor pooled, int64_t B, int64_t N) {
     c10::cuda::CUDAGuard guard(xn.device());
@@ -334,6 +354,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("gelu_fwd", &gelu_fwd);
     m.def("dgelu_mul", &dgelu_mul);
     m.def("dropout", &dropout);
+    m.def("drop_path_scale", &drop_path_scale);
+    m.def("drop_path_bwd", &drop_path_bwd);
     m.def("meanpool_fwd", &meanpool_fwd);
     m.def("meanpool_bwd", &meanpool_bwd);
     m.def("colsum", &colsum);

@@ -500,6 +500,59 @@ __global__ void __launch_bounds__(256) dropout_kernel(const __nv_bfloat16* __res
 }
 
 // ------------------------------------------------------------------------------------------------
+// Stochastic depth (timm drop_path): one keep / drop draw per sample of a residual branch.  Sample g (the global index
+// sample_offset + b, so that ranks draw disjoint samples) is kept iff keep bit g % 8 of dropout_keep8(g / 8, key,
+// thresh16) is set: the same Philox stream, 16-bit quantisation and scale as the dropout kernel, so the effective keep
+// probability is 1 - thresh16 / 65536.  The per-sample scale vector (0 or dropout_scale) feeds the row scale of the
+// branch's last GEMM in the forward and drop_path_bwd in the backward.
+// ------------------------------------------------------------------------------------------------
+__global__ void drop_path_scale_kernel(float* __restrict__ scale, int B, int64_t sample_offset, uint32_t key_lo,
+                                       uint32_t key_hi, uint32_t thresh16, float keep_scale) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const uint64_t g = static_cast<uint64_t>(sample_offset) + static_cast<uint64_t>(b);
+    const uint32_t bits = dropout_keep8(g / 8, key_lo, key_hi, thresh16);
+    scale[b] = ((bits >> (g % 8)) & 1u) ? keep_scale : 0.f;
+}
+
+// dt = bf16(scale[row / N] * dy) and fp32 column sums of the rounded dt (the bias gradient of the branch's last linear
+// layer) in one pass.  Same layout as colsum_kernel: a thread owns one 8-column vector of a slab of rows; four rows are
+// loaded before any is processed so that each thread keeps four 16-byte loads in flight.
+__global__ void __launch_bounds__(256) drop_path_bwd_kernel(const __nv_bfloat16* __restrict__ dy,
+                                                            const float* __restrict__ scale,
+                                                            __nv_bfloat16* __restrict__ dt, float* __restrict__ colsum,
+                                                            int64_t rows, int C, int N, int rows_per_cta) {
+    const int vec = blockIdx.x * blockDim.x + threadIdx.x;
+    if (vec * 8 >= C) return;
+    const int64_t r0 = static_cast<int64_t>(blockIdx.y) * rows_per_cta;
+    const int64_t r1 = min(rows, r0 + rows_per_cta);
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    auto row = [&](const uint4& in, int64_t r) {
+        const float s = __ldg(scale + r / N);
+        float f[8];
+        unpack8(in, f);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) f[q] *= s;
+        const uint4 out = pack8(f);
+        *reinterpret_cast<uint4*>(dt + r * C + vec * 8) = out;
+        unpack8(out, f);  // the column sums are those of the rounded gradient the GEMMs consume
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[q] += f[q];
+    };
+    int64_t r = r0;
+    for (; r + 4 <= r1; r += 4) {
+        uint4 in[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) in[u] = __ldg(reinterpret_cast<const uint4*>(dy + (r + u) * C + vec * 8));
+#pragma unroll
+        for (int u = 0; u < 4; ++u) row(in[u], r + u);
+    }
+    for (; r < r1; ++r) row(__ldg(reinterpret_cast<const uint4*>(dy + r * C + vec * 8)), r);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) atomicAdd(colsum + vec * 8 + q, acc[q]);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Token mean-pool of the head (reference run_vit_training.py:161: x.mean(dim=1) after the final norm) and its backward.
 // Forward: pooled[b, :] = mean_n xn[b, n, :] -- a CTA column-strip sums the N tokens of one image in fp32.
 // Backward: d xn[b, n, :] = dpooled[b, :] / N for every token; written as the broadcast rows the final-LayerNorm
@@ -1254,6 +1307,33 @@ void dropout(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, float p, uint6
     dropout_kernel<<<grid, 256, 0, stream>>>(x, y, n / 8, static_cast<uint32_t>(key), static_cast<uint32_t>(key >> 32),
                                             thresh, dropout_scale(thresh));
     check_launch("dropout");
+}
+
+void drop_path_scale(float* scale, int B, int64_t sample_offset, float p, uint64_t key, cudaStream_t stream) {
+    if (!(p >= 0.f && p < 1.f)) throw std::runtime_error("drop_path_scale: p must be in [0, 1)");
+    if (B < 0 || sample_offset < 0) throw std::runtime_error("drop_path_scale: B and sample_offset must be >= 0");
+    if (B == 0) return;
+    const uint32_t thresh = dropout_thresh16(p);
+    drop_path_scale_kernel<<<(B + 127) / 128, 128, 0, stream>>>(scale, B, sample_offset, static_cast<uint32_t>(key),
+                                                                static_cast<uint32_t>(key >> 32), thresh,
+                                                                dropout_scale(thresh));
+    check_launch("drop_path_scale");
+}
+
+void drop_path_bwd(const __nv_bfloat16* dy, const float* scale, __nv_bfloat16* dt, float* colsum, int64_t rows, int C,
+                   int N, cudaStream_t stream) {
+    if (C % 8 != 0) throw std::runtime_error("drop_path_bwd: width must be a multiple of 8");
+    if (N < 1 || rows % N != 0) throw std::runtime_error("drop_path_bwd: rows must be a whole number of N-row samples");
+    if ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dt)) & 15)
+        throw std::runtime_error("drop_path_bwd: dy and dt must be 16-byte aligned");
+    if (rows == 0) return;
+    const int gx = (C / 8 + 255) / 256;
+    int slabs = std::max(1, (sm_count() * 4) / gx);
+    int rows_per = static_cast<int>((rows + slabs - 1) / slabs);
+    if (rows_per < 1) rows_per = 1;
+    slabs = static_cast<int>((rows + rows_per - 1) / rows_per);
+    drop_path_bwd_kernel<<<dim3(gx, slabs), 256, 0, stream>>>(dy, scale, dt, colsum, rows, C, N, rows_per);
+    check_launch("drop_path_bwd");
 }
 
 void meanpool_fwd(const __nv_bfloat16* xn, __nv_bfloat16* pooled, int B, int N, int D, cudaStream_t stream) {

@@ -36,6 +36,12 @@ void dgelu_mul(const __nv_bfloat16* dg, const __nv_bfloat16* u, __nv_bfloat16* d
 // y = x * keep / (1 - p), keep = Philox-4x32-10(key, vector index): a pure function of (key, position), so recompute and
 // backward regenerate the mask.  p is quantised to 1/65536.  y may alias x.
 void dropout(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, float p, uint64_t key, cudaStream_t stream);
+// Stochastic depth: scale[b] = dropout_scale or 0 for sample sample_offset + b, drawn from the dropout kernel's Philox
+// stream (keep bit g % 8 of vector g / 8).  Effective keep probability 1 - thresh16(p) / 65536.
+void drop_path_scale(float* scale, int B, int64_t sample_offset, float p, uint64_t key, cudaStream_t stream);
+// dt[r, :] = bf16(scale[r / N] * dy[r, :]); colsum (fp32 [C], atomically added to: zero it first) += column sums of dt.
+void drop_path_bwd(const __nv_bfloat16* dy, const float* scale, __nv_bfloat16* dt, float* colsum, int64_t rows, int C,
+                   int N, cudaStream_t stream);
 // pooled[b] = mean over the N tokens of image b; backward broadcasts dpooled[b] / N to every token row.
 void meanpool_fwd(const __nv_bfloat16* xn, __nv_bfloat16* pooled, int B, int N, int D, cudaStream_t stream);
 void meanpool_bwd(const __nv_bfloat16* dpooled, __nv_bfloat16* dxn, int B, int N, int D, cudaStream_t stream);

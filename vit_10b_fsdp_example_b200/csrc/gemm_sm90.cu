@@ -1,7 +1,7 @@
 // Persistent, warp-specialised bf16 GEMM for sm_90a (H100):
 //   TMA (cp.async.bulk.tensor, SWIZZLE_128B)  ->  shared-memory ring (mbarrier full / empty pairs)
 //   wgmma.mma_async m64 x BLOCK_N x 16, two consumer warpgroups per CTA, fp32 accumulators in registers
-//   fused epilogue (bias, exact GELU, dGELU, residual add, pre-activation side output,
+//   fused epilogue (bias, exact GELU, dGELU, per-row scale, residual add, pre-activation side output,
 //   bias-gradient column sums)  ->  swizzled smem  ->  TMA store.
 //
 // One CTA owns a 128 x BLOCK_N output tile; a producer warp (with a reduced register budget) keeps the ring
@@ -120,7 +120,7 @@ __device__ __forceinline__ float dgelu_erf(float x) {
 //                producer's multicast writes stage s of the peer as well and may start only once both released it.
 // Both CTAs walk the same tile sequence, so they fill and drain the ring in lock step; cluster syncs after barrier
 // init and before exit keep a CTA from multicasting into, or arriving on, a peer that has not started or has left.
-template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM>
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM, bool kRowScale>
 __global__ void __launch_bounds__(kNumThreads, 1)
     gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                           const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_aux,
@@ -372,6 +372,15 @@ __global__ void __launch_bounds__(kNumThreads, 1)
                 ext0 = e.residual + static_cast<int64_t>(e.res_row_mod > 0 ? row0 % e.res_row_mod : row0) * e.ld_res;
                 ext1 = e.residual + static_cast<int64_t>(e.res_row_mod > 0 ? row1 % e.res_row_mod : row1) * e.ld_res;
             }
+            // kRowScale (stochastic depth): v = (acc + bias) * row_scale[row / rows_per_scale] before the residual add,
+            // the scale read once per accumulator row of the tile.  A template flag rather than a run-time branch: the
+            // GELU / dGELU epilogues run at the register limit, and any change to their code changes how ptxas
+            // schedules them; the instantiations without the flag compile exactly as they would without the feature.
+            float rs0 = 1.f, rs1 = 1.f;
+            if constexpr (kRowScale) {
+                if (row0_ok) rs0 = __ldg(e.row_scale + row0 / e.rows_per_scale);
+                if (row1_ok) rs1 = __ldg(e.row_scale + row1 / e.rows_per_scale);
+            }
 #pragma unroll
             for (int c = 0; c < BLOCK_N / 64; ++c) {
                 const int ncol0 = n0 + c * 64;
@@ -412,6 +421,9 @@ __global__ void __launch_bounds__(kNumThreads, 1)
                     } else if (ext_is_aux) {
                         v[0] *= dgelu_erf(bf16_lo(x0)), v[1] *= dgelu_erf(bf16_hi(x0));
                         v[2] *= dgelu_erf(bf16_lo(x1)), v[3] *= dgelu_erf(bf16_hi(x1));
+                    }
+                    if constexpr (kRowScale) {  // host: only with kActNone, so this is (acc + bias) * scale
+                        v[0] *= rs0, v[1] *= rs0, v[2] *= rs1, v[3] *= rs1;
                     }
                     if (e.residual != nullptr && !ext_is_aux) {
                         v[0] += bf16_lo(x0), v[1] += bf16_hi(x0), v[2] += bf16_lo(x1), v[3] += bf16_hi(x1);
@@ -562,12 +574,12 @@ void check(cudaError_t err, const char* what) {
     if (err != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(err));
 }
 
-template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM>
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM, bool kRowScale = false>
 void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, const GemmOperand* aux, int M, int N,
             int K, const GemmEpilogue& epi, int max_ctas, cudaStream_t stream, const GemmAgFuse* ag) {
     constexpr int kSmem = kCdBufs * kCdBufBytes + kStages * (kBlockM + BLOCK_N) * kBlockK * 2 + 2 * kStages * 8;
     static_assert(kSmem <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
-    auto kern = gemm_bf16_sm90_kernel<kMajorA, kMajorB, BLOCK_N, kStages, kClusterM>;
+    auto kern = gemm_bf16_sm90_kernel<kMajorA, kMajorB, BLOCK_N, kStages, kClusterM, kRowScale>;
     static bool attr_set = false;
     if (!attr_set) {
         check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem), "cudaFuncSetAttribute");
@@ -653,6 +665,22 @@ void gemm_bf16(const GemmOperand& A, int major_a, const GemmOperand& B, int majo
     if (block_n == 0) block_n = (N > 128) ? 256 : 128;
     // Auto is one CTA per tile: CTA pairs are no faster on the ViT-10B block GEMMs (measurements in DESIGN.md).
     if (cluster == 0 || max_ctas == 1) cluster = 1;
+    if (epi.row_scale != nullptr) {  // the forward of a linear layer: instantiated for K-major A and B only
+        if (epi.rows_per_scale < 1) throw std::runtime_error("gemm: row_scale needs rows_per_scale >= 1");
+        if (epi.act != kActNone || epi.has_aux_out || aux_out != nullptr || epi.colsum != nullptr ||
+            D.nb_inner * D.nb_outer > 1)
+            throw std::runtime_error("gemm: row_scale only with no activation, no aux output, no column sums, unbatched");
+        if (major_a != 0 || major_b != 0) throw std::runtime_error("gemm: row_scale needs K-major A and B");
+        if (block_n == 256)
+            cluster == 2 ? launch<0, 0, 256, 4, 2, true>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag)
+                         : launch<0, 0, 256, 4, 1, true>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
+        else if (block_n == 128)
+            cluster == 2 ? launch<0, 0, 128, 6, 2, true>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag)
+                         : launch<0, 0, 128, 6, 1, true>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
+        else
+            throw std::runtime_error("gemm: unsupported block_n");
+        return;
+    }
 #define B200_DISPATCH(MA, MB, BN, ST)                                                             \
     if (major_a == MA && major_b == MB && block_n == BN) {                                        \
         if (cluster == 2)                                                                         \

@@ -30,6 +30,11 @@ struct GemmEpilogue {
     int res_row_mod = 0;  // > 0: residual row = m % res_row_mod (broadcast a [rows, N] table, e.g. pos_embed)
     int act = kActNone;
     int has_aux_out = 0;  // also store the pre-activation (after bias) through the aux tensor map
+    // [ceil(M / rows_per_scale)] fp32: v = (acc + bias) * row_scale[m / rows_per_scale], before the residual add.
+    // Per-sample scales of stochastic depth (rows_per_scale = tokens per image).  Only with kActNone, no aux output,
+    // no column sums and unbatched problems.
+    const float* row_scale = nullptr;
+    int rows_per_scale = 0;
 };
 
 // All-gather fused into the GEMM (B operand = an FSDP-sharded weight, rank r owns rows [r*rows_per_slab, ...)):

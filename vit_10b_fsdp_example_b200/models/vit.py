@@ -3,7 +3,10 @@
 Architecture parity with the reference model (run_vit_training.py:99-162, timm 0.4.12 blocks):
   * PatchEmbed = Conv2d(3, D, k=s=P) -> tokens; learned pos_embed; dropout           (:124-129,156-157)
   * num_blocks pre-LN blocks: x += proj(attn(norm1(x))); x += fc2(gelu(fc1(norm2(x))))  (:133-141)
-    - LayerNorm eps 1e-5 inside blocks, qkv_bias=True, exact (erf) GELU, no drop-path
+    - LayerNorm eps 1e-5 inside blocks, qkv_bias=True, exact (erf) GELU
+    - optional stochastic depth (timm drop_path, off in the reference): x += drop_path(branch) for both branches,
+      one Bernoulli per sample and branch, kept samples scaled by 1 / keep_prob, block i at rate
+      linspace(0, drop_path_rate, num_blocks)[i], nothing dropped in eval
   * final LayerNorm(eps=1e-6), mean-pool over tokens (no CLS token), Linear head      (:151-153,159-161)
 Parameter names are timm-compatible (``norm1.weight``, ``attn.qkv.weight``, ``mlp.fc1.bias`` ...).
 
@@ -14,6 +17,7 @@ the flat per-unit gradient buffer.  ``ops`` is either ``torch_ops`` (reference, 
 """
 from __future__ import annotations
 
+import functools
 import math
 from typing import Dict, List, Optional, Tuple
 
@@ -108,9 +112,23 @@ class DropoutCtx:
         self.seed = seed
         self.step = 0
         self.training = True
+        # Global index of this rank's first sample (rank * local batch).  The per-sample masks of stochastic depth are
+        # drawn at the global index, so image b of every rank gets its own draw and the masks do not depend on the
+        # world size.  (The element-dropout keys above do not depend on the rank.)
+        self.sample_offset = 0
 
     def key(self, site: int) -> int:
         return (((self.seed * 1000003 + self.step) * 1000003 + site) * 0x9E3779B97F4A7C15) & 0x7FFFFFFFFFFFFFFF
+
+
+@functools.lru_cache(maxsize=None)
+def _drop_path_rates(rate: float, depth: int) -> Tuple[float, ...]:
+    return tuple(float(r) for r in torch.linspace(0, rate, depth))
+
+
+def drop_path_rates(cfg: ViTConfig) -> List[float]:
+    """Stochastic-depth rate of every block: torch.linspace(0, drop_path_rate, num_blocks), like timm's ViT."""
+    return list(_drop_path_rates(float(cfg.drop_path_rate), int(cfg.num_blocks)))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -134,6 +152,16 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     pa, pm = cfg.att_dropout, cfg.mlp_dropout
     use_drop = drop is not None and drop.training and (pa > 0 or pm > 0)
     site = block_idx * 8
+    # Stochastic depth: per-sample scales (0 or 1 / keep_prob) of the attention and MLP branches, applied as a row scale
+    # in the epilogue of the branch's last GEMM.  Regenerated by a checkpoint recompute from the same keys.
+    dpath = None
+    if drop is not None and drop.training and cfg.drop_path_rate > 0:
+        rate = drop_path_rates(cfg)[block_idx]
+        if rate > 0:
+            dpath = (ops.drop_path_scale(drop.key(site + 4), rate, B, drop.sample_offset, x.device),
+                     ops.drop_path_scale(drop.key(site + 5), rate, B, drop.sample_offset, x.device))
+    rs_att = dict(row_scale=dpath[0], rows_per_scale=N) if dpath is not None else {}
+    rs_mlp = dict(row_scale=dpath[1], rows_per_scale=N) if dpath is not None else {}
     ag = getattr(p, "ag", None) or {}  # weights whose all-gather is fused into the GEMM that consumes them
     h1, m1, r1 = ops.ln_fwd(x, p["norm1.weight"], p["norm1.bias"], BLOCK_LN_EPS)
     qkv = ops.linear_fwd(h1, p["attn.qkv.weight"], p["attn.qkv.bias"], ag=ag.get("attn.qkv.weight"))
@@ -157,10 +185,10 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     if use_drop and pm > 0:
         # timm feeds `drop` to both proj_drop and the two MLP dropouts
         masks["proj"] = drop.key(site + 1)
-        t = ops.linear_fwd(a, p["attn.proj.weight"], p["attn.proj.bias"])
-        x1 = x + ops.dropout(t, pm, masks["proj"])
+        t = ops.linear_fwd(a, p["attn.proj.weight"], p["attn.proj.bias"], **rs_att)
+        x1 = x + ops.dropout(t, pm, masks["proj"])  # the per-sample row scale commutes with the element mask
     else:
-        x1 = ops.linear_fwd(a, p["attn.proj.weight"], p["attn.proj.bias"], residual=x)
+        x1 = ops.linear_fwd(a, p["attn.proj.weight"], p["attn.proj.bias"], residual=x, **rs_att)
     h2, m2, r2 = ops.ln_fwd(x1, p["norm2.weight"], p["norm2.bias"], BLOCK_LN_EPS)
     if do_save:
         g, u = ops.linear_fwd(h2, p["mlp.fc1.weight"], p["mlp.fc1.bias"], act="gelu", want_preact=True,
@@ -171,13 +199,15 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
         masks["fc1"] = drop.key(site + 2)
         masks["fc2"] = drop.key(site + 3)
         g = ops.dropout(g, pm, masks["fc1"])
-        t = ops.linear_fwd(g, p["mlp.fc2.weight"], p["mlp.fc2.bias"])
+        t = ops.linear_fwd(g, p["mlp.fc2.weight"], p["mlp.fc2.bias"], **rs_mlp)
         y = x1 + ops.dropout(t, pm, masks["fc2"])
     else:
-        y = ops.linear_fwd(g, p["mlp.fc2.weight"], p["mlp.fc2.bias"], residual=x1)
+        y = ops.linear_fwd(g, p["mlp.fc2.weight"], p["mlp.fc2.bias"], residual=x1, **rs_mlp)
     if not do_save:
         return y, None
     saved = dict(x=x, m1=m1, r1=r1, qkv=qkv, a=a, x1=x1, m2=m2, r2=r2, u=u, masks=masks, lse=lse)
+    if dpath is not None:
+        saved["dpath"] = dpath
     if "P" in extras and lse is None:
         saved["P"] = P
     if "h" in extras:
@@ -197,8 +227,13 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     N, H, hd = cfg.num_patches, cfg.num_heads, cfg.head_dim
     pa, pm = cfg.att_dropout, cfg.mlp_dropout
     masks = s["masks"]
+    dpath = s.get("dpath")  # stochastic depth: per-sample scales of the (attention, MLP) branches, or None
     # ---- MLP ----
-    if "fc2" in masks:
+    if dpath is not None:  # the branch gradient is scaled per sample; the residual gradient dy stays as it is
+        dt = ops.dropout(dy, pm, masks["fc2"]) if "fc2" in masks else dy
+        dt, db2 = ops.drop_path_bwd(dt, dpath[1], N)
+        G["mlp.fc2.bias"].copy_(db2)
+    elif "fc2" in masks:
         dt = ops.dropout(dy, pm, masks["fc2"])
         G["mlp.fc2.bias"].copy_(ops.colsum(dt))
     else:
@@ -230,7 +265,11 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     G["norm2.weight"].copy_(dn2w)
     G["norm2.bias"].copy_(dn2b)
     # ---- attention ----
-    if "proj" in masks:
+    if dpath is not None:
+        dt = ops.dropout(dx1, pm, masks["proj"]) if "proj" in masks else dx1
+        dt, dbp = ops.drop_path_bwd(dt, dpath[0], N)
+        G["attn.proj.bias"].copy_(dbp)
+    elif "proj" in masks:
         dt = ops.dropout(dx1, pm, masks["proj"])
         G["attn.proj.bias"].copy_(ops.colsum(dt))
     else:

@@ -9,6 +9,8 @@ Every function launches hand-written kernels from ``_C.so``:
     (the kernels regenerate the Philox mask of ``dropout`` in registers).  The un-fused path (batched wgmma GEMMs +
     softmax / softmax-backward kernels with materialised P) remains for B200_FUSED_ATTN_BWD=0 and unsupported shapes.
   * LayerNorm fwd/bwd, cross-entropy, im2col, column sums, sum of squares, fused AdamW.
+  * stochastic depth: per-sample Philox scales (``drop_path_scale``), applied as a row scale in the proj / fc2 GEMM
+    epilogues, and ``drop_path_bwd`` (scaled branch gradient + its bias gradient in one pass).
 
 What each group replaces in the reference (all of it reached through timm / torch_xla there):
   linear_fwd / dgrad / wgrad      nn.Linear in timm Attention.qkv / proj, Mlp.fc1 / fc2, the head (run_vit_training.py:134-141,153)
@@ -117,10 +119,11 @@ def _bias_ok(b: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
 
 def gemm_raw(a, lda, major_a, b, ldb, major_b, d, ldd, M, N, K, *, bias=None, residual=None, ld_res=0,
              res_row_mod=0, aux_in=None, ld_aux=0, aux_out=None, ld_aux_out=0, colsum=None, colsum_bi_stride=0,
-             act=ACT_NONE, batch=(), block_n=0, cluster=None, max_ctas=None, ag=()):
+             act=ACT_NONE, batch=(), block_n=0, cluster=None, max_ctas=None, ag=(), row_scale=None, rows_per_scale=0):
     _C.gemm(a, lda, major_a, b, ldb, major_b, d, ldd, M, N, K, bias, residual, ld_res, res_row_mod, aux_in, ld_aux,
             aux_out, ld_aux_out, colsum, colsum_bi_stride, act, list(batch), block_n,
-            _gemm_cluster if cluster is None else cluster, _max_ctas if max_ctas is None else max_ctas, list(ag))
+            _gemm_cluster if cluster is None else cluster, _max_ctas if max_ctas is None else max_ctas, list(ag),
+            row_scale, rows_per_scale)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -147,11 +150,16 @@ def ln_bwd(dy, x, w, mean, rstd, dres=None, want_dxsum: bool = False):
 # Linear
 # ------------------------------------------------------------------------------------------------
 def linear_fwd(x, w, bias=None, act: Optional[str] = None, residual=None, res_row_mod: int = 0,
-               want_preact: bool = False, ag=None):
+               want_preact: bool = False, ag=None, row_scale=None, rows_per_scale: int = 0):
     """ag: optional all-gather fusion spec (see Sm100Backend.ag_fuse_spec): the kernel itself pulls the peers'
-    shards of `w` over NVLink while it computes."""
+    shards of `w` over NVLink while it computes.
+    row_scale: fp32 [M / rows_per_scale] per-sample scales (stochastic depth), applied in the epilogue as
+    (x w^T + bias) * row_scale[m / rows_per_scale] before the residual add; only without an activation."""
     M, K = x.shape
     N = w.shape[0]
+    if row_scale is not None:
+        assert act is None and not want_preact and rows_per_scale > 0, "row_scale: plain linear layers only"
+        assert row_scale.dtype == torch.float32 and row_scale.numel() * rows_per_scale == M, "one scale per sample"
     if act == "gelu" and K < FUSE_ACT_MIN_K and N % 8 == 0 and ag is None:
         # short K: the activation math would not fit under a tile's MMA time -> plain GEMM + memory-bound GELU
         pre = linear_fwd(x, w, bias, residual=None)
@@ -166,7 +174,8 @@ def linear_fwd(x, w, bias=None, act: Optional[str] = None, residual=None, res_ro
     pre = torch.empty(M, ldy, dtype=x.dtype, device=x.device) if want_preact else None
     gemm_raw(x, _ld(x), 0, w, _ld(w), 0, y, ldy, M, N, K, bias=_bias_ok(bias), residual=residual,
              ld_res=_ld(residual) if residual is not None else 0, res_row_mod=res_row_mod, aux_out=pre,
-             ld_aux_out=ldy, act=ACT_GELU if act == "gelu" else ACT_NONE, ag=ag or ())
+             ld_aux_out=ldy, act=ACT_GELU if act == "gelu" else ACT_NONE, ag=ag or (), row_scale=row_scale,
+             rows_per_scale=rows_per_scale)
     if ldy != N:
         y = y[:, :N].contiguous()
         pre = pre[:, :N].contiguous() if pre is not None else None
@@ -232,6 +241,23 @@ def dropout(x, p: float, key: int):
     y = torch.empty_like(xc)
     _C.dropout(xc, y, float(p), int(key) & 0x7FFFFFFFFFFFFFFF)
     return y
+
+
+def drop_path_scale(key: int, p: float, B: int, offset: int, device):
+    """Stochastic depth: fp32 [B], entry b = 0 (sample offset + b dropped) or dropout_scale (kept).  Same bits as
+    ``torch_ops.drop_path_scale``."""
+    scale = torch.empty(B, dtype=torch.float32, device=device)
+    _C.drop_path_scale(scale, int(offset), float(p), _drop_key(key))
+    return scale
+
+
+def drop_path_bwd(dy, scale, N: int):
+    """(dt = bf16(scale[row / N] * dy), fp32 column sums of dt) in one pass."""
+    dyc = dy.contiguous()
+    dt = torch.empty_like(dyc)
+    cs = torch.zeros(dyc.shape[1], dtype=torch.float32, device=dyc.device)
+    _C.drop_path_bwd(dyc, scale, dt, cs, int(N))
+    return dt, cs
 
 
 def mean_pool(xn, B: int, N: int):

@@ -11,6 +11,7 @@ from __future__ import annotations
 import math
 from typing import Optional
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -74,8 +75,10 @@ def dgelu(u):
 
 
 def linear_fwd(x, w, bias=None, act: Optional[str] = None, residual=None, res_row_mod: int = 0,
-               want_preact: bool = False, ag=None):
-    """y = act(x @ w.T + bias) + residual.  residual rows may be broadcast with period res_row_mod."""
+               want_preact: bool = False, ag=None, row_scale=None, rows_per_scale: int = 0):
+    """y = act(x @ w.T + bias) + residual.  residual rows may be broadcast with period res_row_mod.
+    row_scale (fp32 [M / rows_per_scale], no activation): y = (x @ w.T + bias) * row_scale[m / rows_per_scale]
+    + residual -- the per-sample scale of stochastic depth."""
     y = _f32(x) @ _f32(w).t()
     if bias is not None:
         y = y + _f32(bias)
@@ -84,6 +87,9 @@ def linear_fwd(x, w, bias=None, act: Optional[str] = None, residual=None, res_ro
         y = gelu(y)
     elif act is not None:
         raise ValueError(act)
+    if row_scale is not None:
+        assert act is None and row_scale.numel() * rows_per_scale == y.shape[0], "one scale per sample"
+        y = y * row_scale.float().repeat_interleave(rows_per_scale)[:, None]
     if residual is not None:
         r = _f32(residual)
         if res_row_mod:
@@ -129,6 +135,64 @@ def dropout(x, p: float, key: int):
     gen.manual_seed(int(key) & 0x7FFFFFFFFFFFFFFF)
     keep = torch.rand(x.shape, generator=gen, device=x.device) >= p
     return (x.float() * keep * (1.0 / (1.0 - p))).to(x.dtype)
+
+
+# ------------------------------------------------------------------------------------------------
+# Stochastic depth (timm drop_path).  The masks are bit-identical to the GPU kernels (csrc/dropout.cuh), so CPU and GPU
+# runs train on the same masks and the kernels can be tested exactly against this reference.
+# ------------------------------------------------------------------------------------------------
+_M32 = np.uint64(0xFFFFFFFF)
+
+
+def philox4x32_10(c0, c1, k0: int, k1: int):
+    """Philox-4x32-10 of csrc/dropout.cuh on uint32 counter arrays (c0, c1), key (k0, k1): returns 4 uint32 arrays."""
+    c0 = np.asarray(c0, dtype=np.uint64)
+    c1 = np.asarray(c1, dtype=np.uint64)
+    c2 = np.full_like(c0, 0x5EED5EED)
+    c3 = np.full_like(c0, 0x0B200B20)
+    k0, k1 = np.uint64(k0 & 0xFFFFFFFF), np.uint64(k1 & 0xFFFFFFFF)
+    for _ in range(10):
+        p0 = np.uint64(0xD2511F53) * c0
+        p1 = np.uint64(0xCD9E8D57) * c2
+        c0, c1, c2, c3 = ((p1 >> np.uint64(32)) ^ c1 ^ k0, p1 & _M32, (p0 >> np.uint64(32)) ^ c3 ^ k1, p0 & _M32)
+        k0 = (k0 + np.uint64(0x9E3779B9)) & _M32
+        k1 = (k1 + np.uint64(0xBB67AE85)) & _M32
+    return tuple(c.astype(np.uint32) for c in (c0, c1, c2, c3))
+
+
+def dropout_thresh16(p: float) -> int:
+    """dropout_thresh16 of csrc/dropout.cuh, in the same fp32 arithmetic."""
+    return int(np.float32(p) * np.float32(65536.0) + np.float32(0.5))
+
+
+def dropout_scale(thresh16: int) -> float:
+    return float(np.float32(1.0) / (np.float32(1.0) - np.float32(thresh16) / np.float32(65536.0)))
+
+
+def drop_path_keep(key: int, p: float, B: int, offset: int) -> np.ndarray:
+    """bool [B]: sample g = offset + b is kept iff keep bit g % 8 of dropout_keep8(g / 8, key, thresh16(p)) is set,
+    i.e. iff 16-bit chunk g % 8 of Philox vector g / 8 is >= thresh16.  Keep probability 1 - thresh16 / 65536."""
+    key = int(key) & 0x7FFFFFFFFFFFFFFF
+    g = np.arange(offset, offset + B, dtype=np.uint64)
+    i = g // np.uint64(8)
+    c = (g % np.uint64(8)).astype(np.int64)
+    r = np.stack(philox4x32_10(i & _M32, i >> np.uint64(32), key & 0xFFFFFFFF, key >> 32))  # [4, B]
+    word = r[c >> 1, np.arange(B)].astype(np.uint32)
+    chunk = (word >> ((c & 1) * 16).astype(np.uint32)) & np.uint32(0xFFFF)
+    return chunk >= dropout_thresh16(p)
+
+
+def drop_path_scale(key: int, p: float, B: int, offset: int, device):
+    """fp32 [B]: dropout_scale(thresh16(p)) for kept samples, 0 for dropped ones."""
+    keep = drop_path_keep(key, p, B, offset)
+    scale = np.where(keep, np.float32(dropout_scale(dropout_thresh16(p))), np.float32(0.0)).astype(np.float32)
+    return torch.from_numpy(scale).to(device)
+
+
+def drop_path_bwd(dy, scale, N: int):
+    """(dt = scale[row / N] * dy rounded to dy's dtype, fp32 column sums of dt)."""
+    dt = (_f32(dy) * scale.float().repeat_interleave(N)[:, None]).to(dy.dtype)
+    return dt, _f32(dt).sum(dim=0)
 
 
 def mean_pool(xn, B: int, N: int):

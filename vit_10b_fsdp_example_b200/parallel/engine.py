@@ -486,6 +486,9 @@ class FSDPViT:
             n_keep = min(self.keep_blocks, len(blocks))
         keep_from = len(blocks) - n_keep if self.grad_ckpt else 0  # blocks >= keep_from are not recomputed
         self.drop.step = self.step_count
+        # global index of this rank's first image (every rank holds the same local batch): stochastic depth draws its
+        # per-sample masks there, in FSDP and in --run_without_fsdp mode alike
+        self.drop.sample_offset = self.rank * B
         self._begin_step()
         if self._fused_sumsq:
             self._sumsq = torch.zeros(1, dtype=torch.float32, device=self.device)
@@ -564,6 +567,7 @@ class FSDPViT:
         self._wait_gather(self.root)
         rp = self.root.layout.param_views(self.root.full)
         drop = self.drop if self.training else None
+        self.drop.sample_offset = self.rank * B
         x, _ = vit.stem_forward(ops, cfg, rp, images, self.dtype, drop)
         for i, u in enumerate(blocks):
             if i + 1 < len(blocks):

@@ -26,9 +26,12 @@ class GraphedTrainStep:
     """
 
     def __init__(self, model, optimizer, clip_grad_norm: float = 0.0, warmup: int = 3):
+        cfg = model.cfg
+        if model.training and cfg.drop_path_rate > 0:
+            raise RuntimeError("CUDA-graph training steps do not support drop_path_rate > 0 "
+                               "(masks are keyed from the host)")
         if not model.is_cuda:
             raise RuntimeError("CUDA graphs need a CUDA model")
-        cfg = model.cfg
         if model.training and (cfg.pos_dropout > 0 or cfg.att_dropout > 0 or cfg.mlp_dropout > 0):
             raise RuntimeError("CUDA-graph training steps do not support dropout > 0 (masks are seeded from the host)")
         if getattr(optimizer, "fused", False):
