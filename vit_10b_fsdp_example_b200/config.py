@@ -71,6 +71,17 @@ def build_arg_parser() -> argparse.ArgumentParser:
     parser.add_argument("--drop_path_rate", type=_drop_path_rate, default=0.0,
                         help="stochastic depth (timm drop_path): block i drops each residual branch per sample with "
                              "rate linspace(0, drop_path_rate, num_blocks)[i]; 0 = off")
+    # ---- batch mixing and label smoothing (timm 0.4.12 Mixup, mode 'batch'; DeiT's defaults are 0.8 / 1.0 / 0.1) ----
+    parser.add_argument("--mixup", type=_non_negative("--mixup"), default=0.0,
+                        help="Mixup Beta(alpha, alpha) parameter; 0 = off")
+    parser.add_argument("--cutmix", type=_non_negative("--cutmix"), default=0.0,
+                        help="CutMix Beta(alpha, alpha) parameter; 0 = off")
+    parser.add_argument("--mixup_prob", type=_probability("--mixup_prob"), default=1.0,
+                        help="probability that a step mixes its batch (when --mixup or --cutmix is on)")
+    parser.add_argument("--mixup_switch_prob", type=_probability("--mixup_switch_prob"), default=0.5,
+                        help="probability of CutMix instead of Mixup when both are on")
+    parser.add_argument("--smoothing", type=_smoothing, default=0.0,
+                        help="label smoothing of the (mixed) training targets; 0 = off")
     return parser
 
 
@@ -78,6 +89,31 @@ def _drop_path_rate(s: str) -> float:
     v = float(s)
     if not 0.0 <= v < 1.0:
         raise argparse.ArgumentTypeError(f"--drop_path_rate must be in [0, 1), got {s}")
+    return v
+
+
+def _non_negative(flag: str):
+    def parse(s: str) -> float:
+        v = float(s)
+        if not (v >= 0.0 and v != float("inf")):
+            raise argparse.ArgumentTypeError(f"{flag} must be a finite number >= 0, got {s}")
+        return v
+    return parse
+
+
+def _probability(flag: str):
+    def parse(s: str) -> float:
+        v = float(s)
+        if not 0.0 <= v <= 1.0:
+            raise argparse.ArgumentTypeError(f"{flag} must be in [0, 1], got {s}")
+        return v
+    return parse
+
+
+def _smoothing(s: str) -> float:
+    v = float(s)
+    if not 0.0 <= v < 1.0:
+        raise argparse.ArgumentTypeError(f"--smoothing must be in [0, 1), got {s}")
     return v
 
 
@@ -98,17 +134,39 @@ class ViTConfig:
     mlp_dropout: float = 0.0
     num_classes: int = 1000
     drop_path_rate: float = 0.0  # stochastic depth; block i uses linspace(0, drop_path_rate, num_blocks)[i]
+    mixup: float = 0.0  # Mixup / CutMix Beta alphas (0 = off), timm Mixup in 'batch' mode
+    cutmix: float = 0.0
+    mixup_prob: float = 1.0  # probability that a step mixes
+    mixup_switch_prob: float = 0.5  # probability of CutMix when both are on
+    smoothing: float = 0.0  # label smoothing of the training targets
 
     def __post_init__(self):
         if not 0.0 <= self.drop_path_rate < 1.0:
             raise ValueError(f"drop_path_rate must be in [0, 1), got {self.drop_path_rate}")
+        for name in ("mixup", "cutmix"):
+            v = getattr(self, name)
+            if not (v >= 0.0 and v != float("inf")):
+                raise ValueError(f"{name} must be a finite number >= 0, got {v}")
+        for name in ("mixup_prob", "mixup_switch_prob"):
+            if not 0.0 <= getattr(self, name) <= 1.0:
+                raise ValueError(f"{name} must be in [0, 1], got {getattr(self, name)}")
+        if not 0.0 <= self.smoothing < 1.0:
+            raise ValueError(f"smoothing must be in [0, 1), got {self.smoothing}")
+
+    @property
+    def mixing(self) -> bool:
+        """True when training steps may mix their batch (Mixup or CutMix on)."""
+        return self.mixup > 0 or self.cutmix > 0
 
     @classmethod
     def from_args(cls, cfg) -> "ViTConfig":
         return cls(image_size=cfg.image_size, patch_size=cfg.patch_size, embed_dim=cfg.embed_dim,
                    num_heads=cfg.num_heads, num_blocks=cfg.num_blocks, mlp_ratio=cfg.mlp_ratio,
                    pos_dropout=cfg.pos_dropout, att_dropout=cfg.att_dropout, mlp_dropout=cfg.mlp_dropout,
-                   num_classes=cfg.num_classes, drop_path_rate=getattr(cfg, "drop_path_rate", 0.0))
+                   num_classes=cfg.num_classes, drop_path_rate=getattr(cfg, "drop_path_rate", 0.0),
+                   mixup=getattr(cfg, "mixup", 0.0), cutmix=getattr(cfg, "cutmix", 0.0),
+                   mixup_prob=getattr(cfg, "mixup_prob", 1.0), mixup_switch_prob=getattr(cfg, "mixup_switch_prob", 0.5),
+                   smoothing=getattr(cfg, "smoothing", 0.0))
 
     @property
     def grid(self) -> int:

@@ -132,23 +132,38 @@ void attention_bwd(Tensor qkv, Tensor dout, Tensor out, Tensor lse, Tensor delta
                         colsum.has_value() ? f32_ptr(*colsum) : nullptr, (float)drop_p, (uint64_t)drop_key);
 }
 
-void cross_entropy(Tensor logits, Tensor target, OptT dlogits, Tensor loss, OptT correct) {
+// lam < 1: mixed targets (row b with row B-1-b); smoothing > 0: label smoothing.  The defaults are the hard loss.
+void cross_entropy(Tensor logits, Tensor target, OptT dlogits, Tensor loss, OptT correct, double lam,
+                   double smoothing) {
     c10::cuda::CUDAGuard guard(logits.device());
     TORCH_CHECK(target.scalar_type() == at::kLong && target.is_cuda(), "target must be a CUDA int64 tensor");
+    TORCH_CHECK(lam >= 0.0 && lam <= 1.0 && smoothing >= 0.0 && smoothing < 1.0,
+                "cross_entropy: lam must be in [0, 1] and smoothing in [0, 1)");
     const int B = (int)logits.size(0), C = (int)logits.size(1);
     b200::cross_entropy(bf16_ptr(logits), reinterpret_cast<const int64_t*>(target.data_ptr()),
                         dlogits.has_value() ? bf16_mut(*dlogits) : nullptr, f32_ptr(loss),
                         correct.has_value() ? reinterpret_cast<int*>(correct->data_ptr()) : nullptr, B, C,
-                        cur_stream());
+                        cur_stream(), lam, smoothing);
 }
 
-void im2col(Tensor img, Tensor cols, int64_t P) {
+// lam given: mix image b with image B-1-b, Mixup with an empty box, CutMix with box = [yl, yh, xl, xh].
+void im2col(Tensor img, Tensor cols, int64_t P, std::optional<double> lam, std::vector<int64_t> box) {
     c10::cuda::CUDAGuard guard(img.device());
     TORCH_CHECK(img.is_contiguous() && img.dim() == 4 && img.size(1) == 3, "images must be contiguous [B,3,S,S]");
     const bool is_bf16 = img.scalar_type() == at::kBFloat16;
     TORCH_CHECK(is_bf16 || img.scalar_type() == at::kFloat, "images must be fp32 or bf16");
+    b200::Im2colMix mix;
+    if (lam.has_value()) {
+        TORCH_CHECK(*lam >= 0.0 && *lam <= 1.0, "im2col: lam must be in [0, 1]");
+        TORCH_CHECK(box.empty() || box.size() == 4, "im2col: box must be [] or [yl, yh, xl, xh]");
+        mix.lam = (float)*lam, mix.mlam = (float)(1.0 - *lam);
+        mix.mode = box.empty() ? 1 : 2;
+        if (!box.empty()) mix.yl = (int)box[0], mix.yh = (int)box[1], mix.xl = (int)box[2], mix.xh = (int)box[3];
+    } else {
+        TORCH_CHECK(box.empty(), "im2col: a CutMix box needs lam");
+    }
     b200::im2col(img.data_ptr(), is_bf16, bf16_mut(cols), (int)img.size(0), (int)img.size(2), (int)P,
-                 (int)cols.size(1), cur_stream());
+                 (int)cols.size(1), cur_stream(), mix);
 }
 
 void gelu_fwd(Tensor u, Tensor g) {
@@ -349,8 +364,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("attention_bwd", &attention_bwd, py::arg("qkv"), py::arg("dout"), py::arg("out"), py::arg("lse"),
           py::arg("delta"), py::arg("dqkv"), py::arg("colsum"), py::arg("B"), py::arg("N"), py::arg("H"), py::arg("hd"),
           py::arg("drop_p") = 0.0, py::arg("drop_key") = 0);
-    m.def("cross_entropy", &cross_entropy);
-    m.def("im2col", &im2col);
+    m.def("cross_entropy", &cross_entropy, py::arg("logits"), py::arg("target"), py::arg("dlogits"), py::arg("loss"),
+          py::arg("correct"), py::arg("lam") = 1.0, py::arg("smoothing") = 0.0);
+    m.def("im2col", &im2col, py::arg("img"), py::arg("cols"), py::arg("P"), py::arg("lam") = py::none(),
+          py::arg("box") = std::vector<int64_t>());
     m.def("gelu_fwd", &gelu_fwd);
     m.def("dgelu_mul", &dgelu_mul);
     m.def("dropout", &dropout);

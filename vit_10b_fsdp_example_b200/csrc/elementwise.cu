@@ -871,14 +871,17 @@ __global__ void __launch_bounds__(256) softmax_bwd_long_kernel(__nv_bfloat16* __
 }
 
 // ------------------------------------------------------------------------------------------------
-// Cross entropy: loss += mean_b( logsumexp(logits_b) - logits_b[target_b] ), dlogits = (softmax - 1hot)/B
-// One CTA per row.
+// Cross entropy against a mixed, smoothed target (timm mixup_target + SoftTargetCrossEntropy):
+//   t_c = off + w1 * [c == y_b] + w2 * [c == y_{B-1-b}],  w1 = (on - off) * lam,  w2 = (on - off) * (1 - lam)
+//   loss += mean_b( logsumexp(logits_b) - off * sum_c logits_bc - w1 * logits_b[y_b] - w2 * logits_b[y_{B-1-b}] )
+//   dlogits = (softmax - t) / B
+// The hard call (w1 = 1, w2 = 0, off = 0) computes exactly the plain cross-entropy expressions.  One CTA per row.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) cross_entropy_kernel(const __nv_bfloat16* __restrict__ logits,
                                                             const int64_t* __restrict__ target,
                                                             __nv_bfloat16* __restrict__ dlogits,
                                                             float* __restrict__ loss, int* __restrict__ correct,
-                                                            int B, int C, float inv_b) {
+                                                            int B, int C, float inv_b, float w1, float w2, float off) {
     __shared__ float red[64];
     __shared__ int red_i[8];
     const int row = blockIdx.x;
@@ -901,20 +904,29 @@ __global__ void __launch_bounds__(256) cross_entropy_kernel(const __nv_bfloat16*
     mx = red[0], arg = red_i[0];
     for (int i = 1; i < blockDim.x / 32; ++i)
         if (red[i] > mx || (red[i] == mx && red_i[i] < arg)) mx = red[i], arg = red_i[i];
-    float s = 0.f, dummy = 0.f;
-    for (int c = threadIdx.x; c < C; c += blockDim.x) s += __expf(__bfloat162float(lr[c]) - mx);
-    block_sum2<256>(s, dummy, red);
+    float s = 0.f, sx = 0.f;  // sum of exp, sum of logits (the smoothing term)
+    for (int c = threadIdx.x; c < C; c += blockDim.x) {
+        const float v = __bfloat162float(lr[c]);
+        s += __expf(v - mx);
+        sx += v;
+    }
+    block_sum2<256>(s, sx, red);
     const float lse = mx + __logf(s);
     const int tgt = static_cast<int>(target[row]);
+    const int tgt2 = w2 != 0.f ? static_cast<int>(target[B - 1 - row]) : tgt;
     if (dlogits != nullptr) {
         __nv_bfloat16* dr = dlogits + static_cast<int64_t>(row) * C;
         for (int c = threadIdx.x; c < C; c += blockDim.x) {
             const float pr = __expf(__bfloat162float(lr[c]) - lse);
-            dr[c] = __float2bfloat16((pr - (c == tgt ? 1.f : 0.f)) * inv_b);
+            const float t = (c == tgt ? w1 : 0.f) + (c == tgt2 ? w2 : 0.f) + off;
+            dr[c] = __float2bfloat16((pr - t) * inv_b);
         }
     }
     if (threadIdx.x == 0) {
-        atomicAdd(loss, (lse - __bfloat162float(lr[tgt])) * inv_b);
+        float picked = w1 * __bfloat162float(lr[tgt]);
+        if (w2 != 0.f) picked += w2 * __bfloat162float(lr[tgt2]);
+        if (off != 0.f) picked += off * sx;
+        atomicAdd(loss, (lse - picked) * inv_b);
         if (correct != nullptr && arg == tgt) atomicAdd(correct, 1);
     }
 }
@@ -922,10 +934,15 @@ __global__ void __launch_bounds__(256) cross_entropy_kernel(const __nv_bfloat16*
 // ------------------------------------------------------------------------------------------------
 // Patch im2col: images [B, 3, S, S] (fp32 or bf16) -> cols [B * (S/P)^2, Kpad] bf16 with
 // k = c * P * P + py * P + px (the Conv2d weight's flattening order); columns >= 3 P^2 are zero.
+// MIX (timm Mixup, mode 'batch', image b paired with image B-1-b):
+//   0  no mixing;
+//   1  Mixup:  x_b * lam + x_{B-1-b} * mlam in fp32, each product and the sum rounded once (no FMA contraction), which
+//      is what the fp32 PyTorch expression x.mul_(lam).add_(x.flip(0).mul_(1 - lam)) computes;
+//   2  CutMix: pixels in [yl, yh) x [xl, xh) come from image B-1-b, all others from image b.
 // ------------------------------------------------------------------------------------------------
-template <typename T>
+template <typename T, int MIX>
 __global__ void im2col_kernel(const T* __restrict__ img, __nv_bfloat16* __restrict__ cols, int B, int S, int P,
-                              int Kpad) {
+                              int Kpad, Im2colMix mix) {
     const int G = S / P;
     const int64_t total = static_cast<int64_t>(B) * G * G * Kpad;
     const int K = 3 * P * P;
@@ -938,7 +955,21 @@ __global__ void im2col_kernel(const T* __restrict__ img, __nv_bfloat16* __restri
             const int c = k / (P * P), rem = k % (P * P), py = rem / P, px = rem % P;
             const int gx = static_cast<int>(patch % G), gy = static_cast<int>((patch / G) % G);
             const int64_t b = patch / (G * G);
-            v = static_cast<float>(img[((b * 3 + c) * S + gy * P + py) * S + gx * P + px]);
+            if constexpr (MIX == 0) {
+                v = static_cast<float>(img[((b * 3 + c) * S + gy * P + py) * S + gx * P + px]);
+            } else {
+                const int y = gy * P + py, x = gx * P + px;
+                const int64_t pix = (static_cast<int64_t>(c) * S + y) * S + x, img_elems = 3LL * S * S;
+                const int64_t b2 = B - 1 - b;
+                if constexpr (MIX == 1) {
+                    const float a = static_cast<float>(img[b * img_elems + pix]);
+                    const float o = static_cast<float>(img[b2 * img_elems + pix]);
+                    v = __fadd_rn(__fmul_rn(a, mix.lam), __fmul_rn(o, mix.mlam));
+                } else {
+                    const bool in_box = y >= mix.yl && y < mix.yh && x >= mix.xl && x < mix.xh;
+                    v = static_cast<float>(img[(in_box ? b2 : b) * img_elems + pix]);
+                }
+            }
         }
         cols[i] = __float2bfloat16(v);
     }
@@ -1267,18 +1298,39 @@ void softmax_bwd(__nv_bfloat16* dp, const __nv_bfloat16* p, int64_t rows, int n,
 }
 
 void cross_entropy(const __nv_bfloat16* logits, const int64_t* target, __nv_bfloat16* dlogits, float* loss,
-                   int* correct, int B, int C, cudaStream_t stream) {
-    cross_entropy_kernel<<<B, 256, 0, stream>>>(logits, target, dlogits, loss, correct, B, C, 1.0f / B);
+                   int* correct, int B, int C, cudaStream_t stream, double lam, double smoothing) {
+    // target weights in double, rounded once: lam = 1, smoothing = 0 gives exactly w1 = 1, w2 = 0, off = 0
+    const double off = smoothing / C, on = 1.0 - smoothing + off;
+    const float w1 = static_cast<float>((on - off) * lam), w2 = static_cast<float>((on - off) * (1.0 - lam));
+    if (w2 != 0.f && B % 2 != 0) throw std::runtime_error("cross_entropy: mixed targets need an even batch");
+    cross_entropy_kernel<<<B, 256, 0, stream>>>(logits, target, dlogits, loss, correct, B, C, 1.0f / B, w1, w2,
+                                                static_cast<float>(off));
     check_launch("cross_entropy");
 }
 
-void im2col(const void* img, bool img_is_bf16, __nv_bfloat16* cols, int B, int S, int P, int Kpad,
-            cudaStream_t stream) {
+template <typename T>
+static void im2col_launch(const T* img, __nv_bfloat16* cols, int B, int S, int P, int Kpad, const Im2colMix& mix,
+                          cudaStream_t stream) {
     const int grid = sm_count() * 8;
-    if (img_is_bf16)
-        im2col_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(img), cols, B, S, P, Kpad);
+    if (mix.mode == 0)
+        im2col_kernel<T, 0><<<grid, 256, 0, stream>>>(img, cols, B, S, P, Kpad, mix);
+    else if (mix.mode == 1)
+        im2col_kernel<T, 1><<<grid, 256, 0, stream>>>(img, cols, B, S, P, Kpad, mix);
     else
-        im2col_kernel<float><<<grid, 256, 0, stream>>>(static_cast<const float*>(img), cols, B, S, P, Kpad);
+        im2col_kernel<T, 2><<<grid, 256, 0, stream>>>(img, cols, B, S, P, Kpad, mix);
+}
+
+void im2col(const void* img, bool img_is_bf16, __nv_bfloat16* cols, int B, int S, int P, int Kpad,
+            cudaStream_t stream, const Im2colMix& mix) {
+    if (mix.mode < 0 || mix.mode > 2) throw std::runtime_error("im2col: mix mode must be 0, 1 or 2");
+    if (mix.mode != 0 && B % 2 != 0) throw std::runtime_error("im2col: batch mixing needs an even batch");
+    if (mix.mode == 2 && !(0 <= mix.yl && mix.yl <= mix.yh && mix.yh <= S && 0 <= mix.xl && mix.xl <= mix.xh &&
+                           mix.xh <= S))
+        throw std::runtime_error("im2col: the CutMix box must lie inside the image");
+    if (img_is_bf16)
+        im2col_launch(static_cast<const __nv_bfloat16*>(img), cols, B, S, P, Kpad, mix, stream);
+    else
+        im2col_launch(static_cast<const float*>(img), cols, B, S, P, Kpad, mix, stream);
     check_launch("im2col");
 }
 

@@ -19,12 +19,20 @@ void softmax_fwd(__nv_bfloat16* s, int64_t rows, int n, int64_t ld, float scale,
 void softmax_bwd(__nv_bfloat16* dp, const __nv_bfloat16* p, int64_t rows, int n, int64_t ld, float scale,
                  cudaStream_t stream);
 
-// loss (fp32 scalar, atomically added) = mean CE; dlogits may be null (eval); correct may be null.
+// loss (fp32 scalar, atomically added) = mean CE; dlogits may be null (eval); correct may be null (counts argmax ==
+// target).  lam < 1 mixes row b's target with that of row B-1-b (B even); smoothing > 0 smooths both (timm
+// mixup_target): the soft target is lam * smooth(y_b) + (1 - lam) * smooth(y_{B-1-b}).
 void cross_entropy(const __nv_bfloat16* logits, const int64_t* target, __nv_bfloat16* dlogits, float* loss,
-                   int* correct, int B, int C, cudaStream_t stream);
+                   int* correct, int B, int C, cudaStream_t stream, double lam = 1.0, double smoothing = 0.0);
 
+// Batch mixing fused into im2col (timm Mixup, mode 'batch'): image b is mixed with image B-1-b (B even).
+struct Im2colMix {
+    int mode = 0;               // 0 none, 1 Mixup (blend with lam / mlam), 2 CutMix (the box comes from image B-1-b)
+    float lam = 1.f, mlam = 0.f;  // Mixup weights: fp32(lam) and fp32(1 - lam), 1 - lam taken in double
+    int yl = 0, yh = 0, xl = 0, xh = 0;  // CutMix box [yl, yh) x [xl, xh) in pixels
+};
 void im2col(const void* img, bool img_is_bf16, __nv_bfloat16* cols, int B, int S, int P, int Kpad,
-            cudaStream_t stream);
+            cudaStream_t stream, const Im2colMix& mix = Im2colMix());
 
 // Wide-row LayerNorm backward as a cp.async.bulk row pipeline (layernorm_stream.cu); same contract as layernorm_bwd.
 bool layernorm_bwd_stream_supported(int D);

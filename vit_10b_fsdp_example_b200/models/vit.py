@@ -7,6 +7,8 @@ Architecture parity with the reference model (run_vit_training.py:99-162, timm 0
     - optional stochastic depth (timm drop_path, off in the reference): x += drop_path(branch) for both branches,
       one Bernoulli per sample and branch, kept samples scaled by 1 / keep_prob, block i at rate
       linspace(0, drop_path_rate, num_blocks)[i], nothing dropped in eval
+  * optional Mixup / CutMix (timm Mixup, mode 'batch', off in the reference): drawn on the host per step (draw_mix),
+    applied inside the patch im2col, with the mixed, smoothed target handled by the cross-entropy
   * final LayerNorm(eps=1e-6), mean-pool over tokens (no CLS token), Linear head      (:151-153,159-161)
 Parameter names are timm-compatible (``norm1.weight``, ``attn.qkv.weight``, ``mlp.fc1.bias`` ...).
 
@@ -21,6 +23,7 @@ import functools
 import math
 from typing import Dict, List, Optional, Tuple
 
+import numpy as np
 import torch
 
 from ..config import ViTConfig
@@ -119,6 +122,47 @@ class DropoutCtx:
 
     def key(self, site: int) -> int:
         return (((self.seed * 1000003 + self.step) * 1000003 + site) * 0x9E3779B97F4A7C15) & 0x7FFFFFFFFFFFFFFF
+
+
+# ------------------------------------------------------------------------------------------------
+# Batch mixing (--mixup / --cutmix): timm 0.4.12 Mixup, mode 'batch', image b paired with image B-1-b
+# ------------------------------------------------------------------------------------------------
+Mix = Tuple[float, Optional[Tuple[int, int, int, int]]]  # (lam, CutMix box (yl, yh, xl, xh) or None for Mixup)
+
+
+def mix_rng(seed: int, step: int, rank: int) -> np.random.Generator:
+    """The host generator of one step's mixing draws: a pure function of (seed, step, rank), so a resumed run draws what
+    an uninterrupted one would.  Each rank draws for itself and mixes within its own local batch (DeiT's per-rank
+    seeding)."""
+    return np.random.default_rng([seed & 0xFFFF_FFFF_FFFF_FFFF, step, rank])
+
+
+def draw_mix(cfg: ViTConfig, rng: np.random.Generator) -> Optional[Mix]:
+    """One step's mixing parameters, drawn like timm's ``Mixup._params_per_batch`` and ``cutmix_bbox_and_lam``
+    (margin 0, correct_lam=True) on ``cfg.image_size`` square images.  None when the step does not mix (lam == 1,
+    which includes a CutMix box of zero area); otherwise ``(lam, None)`` for Mixup or ``(lam, (yl, yh, xl, xh))`` for
+    CutMix."""
+    if not cfg.mixing:
+        return None
+    if not rng.random() < cfg.mixup_prob:
+        return None
+    if cfg.mixup > 0 and cfg.cutmix > 0:
+        use_cutmix = rng.random() < cfg.mixup_switch_prob
+    else:
+        use_cutmix = cfg.cutmix > 0
+    alpha = cfg.cutmix if use_cutmix else cfg.mixup
+    lam = float(rng.beta(alpha, alpha))
+    box = None
+    if use_cutmix:
+        S = cfg.image_size
+        cut = int(S * np.sqrt(1 - lam))
+        cy = int(rng.integers(0, S))
+        cx = int(rng.integers(0, S))
+        yl, yh = int(np.clip(cy - cut // 2, 0, S)), int(np.clip(cy + cut // 2, 0, S))
+        xl, xh = int(np.clip(cx - cut // 2, 0, S)), int(np.clip(cx + cut // 2, 0, S))
+        lam = 1.0 - (yh - yl) * (xh - xl) / float(S * S)
+        box = (yl, yh, xl, xh)
+    return None if lam == 1.0 else (lam, box)
 
 
 @functools.lru_cache(maxsize=None)
@@ -307,9 +351,13 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
 # ------------------------------------------------------------------------------------------------
 # Stem (patch embed + pos embed) and head (final norm, mean pool, classifier, loss)
 # ------------------------------------------------------------------------------------------------
-def stem_forward(ops, cfg: ViTConfig, p, images, dtype, drop: Optional[DropoutCtx] = None):
+def stem_forward(ops, cfg: ViTConfig, p, images, dtype, drop: Optional[DropoutCtx] = None, mix: Optional[Mix] = None):
+    """mix: this step's batch mixing (``draw_mix``), applied inside the im2col; the saved cols are the mixed patches."""
     B = images.shape[0]
-    cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype)
+    if mix is None:
+        cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype)
+    else:
+        cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype, mix=mix)
     x0 = ops.linear_fwd(cols, p["patch_embed.proj.weight"], p["patch_embed.proj.bias"], residual=p["pos_embed"],
                         res_row_mod=cfg.num_patches)
     mask = None  # dropout key of the position-embedding dropout (reference :129,157)

@@ -416,19 +416,30 @@ def attention_bwd(dout, qkv, p, B: int, N: int, H: int, hd: int, want_colsum: bo
 # ------------------------------------------------------------------------------------------------
 # Patch embedding, loss
 # ------------------------------------------------------------------------------------------------
-def patch_im2col(images, P: int, kpad: int, dtype):
+def patch_im2col(images, P: int, kpad: int, dtype, mix=None):
+    """mix = (lam, box) from vit.draw_mix: Mixup (box None) or CutMix of image b with image B-1-b, fused into the
+    im2col (torch_ops.mix_images is the reference)."""
     B, _, S, _ = images.shape
     G = S // P
     cols = torch.empty(B * G * G, kpad, dtype=dtype, device=images.device)
-    _C.im2col(images.contiguous(), cols, P)
+    if mix is None:
+        _C.im2col(images.contiguous(), cols, P)
+    else:
+        lam, box = mix
+        _C.im2col(images.contiguous(), cols, P, float(lam), list(box) if box is not None else [])
     return cols
 
 
-def cross_entropy(logits, target, want_grad: bool = True):
+def cross_entropy(logits, target, want_grad: bool = True, mix=None, smoothing: float = 0.0):
+    """mix / smoothing: the soft target lam * smooth(y_b) + (1 - lam) * smooth(y_{B-1-b}) (timm mixup_target)."""
     loss = torch.zeros(1, dtype=torch.float32, device=logits.device)
     correct = torch.zeros(1, dtype=torch.int32, device=logits.device)
     dlogits = torch.empty_like(logits) if want_grad else None
-    _C.cross_entropy(logits, target, dlogits, loss, correct)
+    if mix is None and smoothing == 0:
+        _C.cross_entropy(logits, target, dlogits, loss, correct)
+    else:
+        lam = 1.0 if mix is None else float(mix[0])
+        _C.cross_entropy(logits, target, dlogits, loss, correct, lam, float(smoothing))
     return loss[0], dlogits, correct[0]
 
 

@@ -294,7 +294,23 @@ def attention_bwd(dout, qkv, p, B: int, N: int, H: int, hd: int, want_colsum: bo
 # ------------------------------------------------------------------------------------------------
 # Patch embedding (timm PatchEmbed = Conv2d(k=s=P)) as im2col + GEMM -- run_vit_training.py:124,156
 # ------------------------------------------------------------------------------------------------
-def patch_im2col(images, P: int, kpad: int, dtype):
+def mix_images(images, mix):
+    """timm 0.4.12 ``Mixup._mix_batch`` (mode 'batch') in fp32 with mix = (lam, box) from ``vit.draw_mix``.
+    Mixup: x * lam + x.flip(0) * (1 - lam), each product and the sum rounded to fp32 (what the fused im2col computes).
+    CutMix: the box (yl, yh, xl, xh) of image b comes from image B-1-b."""
+    lam, box = mix
+    x = images.float()
+    if box is None:
+        return x * lam + x.flip(0) * (1.0 - lam)
+    yl, yh, xl, xh = box
+    x = x.clone()
+    x[:, :, yl:yh, xl:xh] = x.flip(0)[:, :, yl:yh, xl:xh]
+    return x
+
+
+def patch_im2col(images, P: int, kpad: int, dtype, mix=None):
+    if mix is not None:
+        images = mix_images(images, mix)
     B, C, S, _ = images.shape
     G = S // P
     cols = images.view(B, C, G, P, G, P).permute(0, 2, 4, 1, 3, 5).reshape(B * G * G, C * P * P)
@@ -305,9 +321,28 @@ def patch_im2col(images, P: int, kpad: int, dtype):
 
 # ------------------------------------------------------------------------------------------------
 # Loss (torch.nn.CrossEntropyLoss, mean) -- run_vit_training.py:229,262 ; eval argmax -- :312-313
+# With mix / smoothing: timm 0.4.12 mixup_target + SoftTargetCrossEntropy (label smoothing alone is DeiT's
+# LabelSmoothingCrossEntropy, i.e. F.cross_entropy(..., label_smoothing=smoothing))
 # ------------------------------------------------------------------------------------------------
-def cross_entropy(logits, target, want_grad: bool = True):
+def mixup_target(target, num_classes: int, lam: float = 1.0, smoothing: float = 0.0):
+    """timm 0.4.12 ``mixup_target``: lam * smooth(onehot(y)) + (1 - lam) * smooth(onehot(y.flip(0))), fp32."""
+    off = smoothing / num_classes
+    on = 1.0 - smoothing + off
+
+    def one_hot(t):
+        return torch.full((t.numel(), num_classes), off, device=t.device).scatter_(1, t.long().view(-1, 1), on)
+
+    return one_hot(target) * lam + one_hot(target.flip(0)) * (1.0 - lam)
+
+
+def cross_entropy(logits, target, want_grad: bool = True, mix=None, smoothing: float = 0.0):
     lf = _f32(logits)
+    if mix is not None or smoothing > 0:
+        soft = mixup_target(target, lf.shape[1], 1.0 if mix is None else mix[0], smoothing)
+        logp = torch.log_softmax(lf, dim=-1)
+        loss = (-soft * logp).sum(dim=-1).mean()
+        dlogits = ((logp.exp() - soft) / lf.shape[0]).to(logits.dtype) if want_grad else None
+        return loss, dlogits, (lf.argmax(dim=-1) == target).sum()
     lse = torch.logsumexp(lf, dim=-1)
     picked = lf.gather(1, target.view(-1, 1)).squeeze(1)
     loss = (lse - picked).mean()

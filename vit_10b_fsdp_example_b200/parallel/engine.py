@@ -489,6 +489,19 @@ class FSDPViT:
         # global index of this rank's first image (every rank holds the same local batch): stochastic depth draws its
         # per-sample masks there, in FSDP and in --run_without_fsdp mode alike
         self.drop.sample_offset = self.rank * B
+        # Mixup / CutMix: one host draw per step, keyed by (seed, step_count, rank); this rank mixes image b with image
+        # B-1-b of its own local batch inside the im2col, and the loss takes the matching soft targets
+        mix = None
+        if cfg.mixing:
+            if B % 2:
+                raise ValueError(f"--mixup / --cutmix pair image b with image B-1-b and need an even local batch, "
+                                 f"got {B}")
+            mix = vit.draw_mix(cfg, vit.mix_rng(self.drop.seed, self.step_count, self.rank))
+        loss_kw = {}
+        if mix is not None:
+            loss_kw["mix"] = mix
+        if cfg.smoothing > 0:
+            loss_kw["smoothing"] = cfg.smoothing
         self._begin_step()
         if self._fused_sumsq:
             self._sumsq = torch.zeros(1, dtype=torch.float32, device=self.device)
@@ -498,7 +511,7 @@ class FSDPViT:
             self._issue_gather(blocks[0], fuse=True)
         self._wait_gather(self.root)
         rp = self.root.layout.param_views(self.root.full)
-        x, stem_saved = vit.stem_forward(ops, cfg, rp, images, self.dtype, self.drop)
+        x, stem_saved = vit.stem_forward(ops, cfg, rp, images, self.dtype, self.drop, mix=mix)
         ckpt: List[torch.Tensor] = []
         saved_all = []
         for i, u in enumerate(blocks):
@@ -517,7 +530,7 @@ class FSDPViT:
             if self.reshard_after_forward and i != len(blocks) - 1:
                 self._release_params(u)  # the last block is needed again immediately by backward
         logits, head_saved = vit.head_forward(ops, cfg, rp, x, B)
-        loss, dlogits, _ = ops.cross_entropy(logits, target, want_grad=True)
+        loss, dlogits, _ = ops.cross_entropy(logits, target, want_grad=True, **loss_kw)
         # -------- backward --------
         rg = self._grad_views(self.root)
         dx, dx_sum = vit.head_backward(ops, cfg, rp, rg, head_saved, dlogits, B)

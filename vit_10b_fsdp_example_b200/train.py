@@ -176,6 +176,10 @@ class Trainer:
     def __init__(self, rt: Runtime, cfg):
         self.rt, self.cfg = rt, cfg
         say = rt.master_print
+        if ViTConfig.from_args(cfg).mixing and (cfg.batch_size // rt.world) % 2:
+            raise ValueError(f"--mixup / --cutmix mix image b with image B-1-b of each rank's batch and need an even "
+                             f"local batch; --batch_size {cfg.batch_size} over {rt.world} ranks gives "
+                             f"{cfg.batch_size // rt.world}")
         (self.train_set, self.train_loader, self.train_sampler,
          _, self.val_loader, _) = build_datasets(cfg, rt.device, rt.world, rt.rank, log=say)
         rt.rendezvous("loaded dataset")
