@@ -13,6 +13,7 @@
 //   sum of squares  -> FSDP.clip_grad_norm_                            (run_vit_training.py:270)
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
+#include <cmath>
 #include <cstdint>
 #include <cstdlib>
 #include <stdexcept>
@@ -1041,8 +1042,11 @@ __global__ void __launch_bounds__(256) adamw_split_kernel(uint16_t* __restrict__
     const float coef = clip_coef != nullptr ? *clip_coef : 1.0f;
     if (hyper != nullptr) {  // lr and step live on the device so the launch can sit inside a CUDA graph
         lr = hyper[0];
-        bc1 = 1.f - powf(beta1, hyper[1]);
-        bc2 = 1.f - powf(beta2, hyper[1]);
+        // 1 - beta^t as -expm1(t * log1p(beta - 1)) (beta - 1 is exact): --use_fast_math turns powf into
+        // ex2.approx(t * lg2.approx(beta)), whose ~1e-7 absolute error in lg2(beta2) is a ~1e-4 relative error in
+        // 1 - beta2^t at small t, i.e. a 5e-5 error in every update of the first steps
+        bc1 = -expm1f(hyper[1] * log1pf(beta1 - 1.f));
+        bc2 = -expm1f(hyper[1] * log1pf(beta2 - 1.f));
     }
     const float inv_bc1 = 1.f / bc1, inv_bc2 = 1.f / bc2, decay = 1.f - lr * wd;
     const int64_t n4 = n / 4;
@@ -1428,8 +1432,9 @@ void adamw_split(uint16_t* hi, int16_t* lo, float* m, float* v, const void* grad
                  cudaStream_t stream, const float* hyper) {
     const int grid = static_cast<int>(std::min<int64_t>((n / 4 + 255) / 256 + 1, sm_count() * 16));
     if (grid == 0) return;
-    const float bc1 = 1.f - powf(beta1, static_cast<float>(step));
-    const float bc2 = 1.f - powf(beta2, static_cast<float>(step));
+    // 1 - beta^t in double: in fp32, 1 - powf(0.999f, 2) keeps only the rounding error of powf (1.5e-5 of 0.002)
+    const float bc1 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta1), static_cast<double>(step)));
+    const float bc2 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta2), static_cast<double>(step)));
     if (grad_is_bf16)
         adamw_split_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(hi, lo, m, v, static_cast<const __nv_bfloat16*>(grad),
                                                                    n, clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2,
@@ -1444,8 +1449,9 @@ void adamw_fp32(float* w, float* m, float* v, const void* grad, bool grad_is_bf1
                 float lr, float beta1, float beta2, float eps, float wd, int step, cudaStream_t stream) {
     const int grid = static_cast<int>(std::min<int64_t>((n + 255) / 256, sm_count() * 16));
     if (grid == 0) return;
-    const float bc1 = 1.f - powf(beta1, static_cast<float>(step));
-    const float bc2 = 1.f - powf(beta2, static_cast<float>(step));
+    // 1 - beta^t in double: in fp32, 1 - powf(0.999f, 2) keeps only the rounding error of powf (1.5e-5 of 0.002)
+    const float bc1 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta1), static_cast<double>(step)));
+    const float bc2 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta2), static_cast<double>(step)));
     if (grad_is_bf16)
         adamw_fp32_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(w, m, v, static_cast<const __nv_bfloat16*>(grad), n,
                                                                   clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2);

@@ -170,12 +170,16 @@ __global__ void __launch_bounds__(kMaxThreads, 1)
                 float r = fmaf(rstd * gam[v][q], df[q], rf[q] + k0);
                 r = fmaf(-k1, xf[q], r);
                 o[q] = r;
-                if constexpr (kDxSum) dxs[v][q] += r;
             }
             uint4 pk;
             pk.x = pack_bf16x2(o[0], o[1]), pk.y = pack_bf16x2(o[2], o[3]);
             pk.z = pack_bf16x2(o[4], o[5]), pk.w = pack_bf16x2(o[6], o[7]);
             dxr[ct + v * ncons] = pk;
+            if constexpr (kDxSum) {
+                unpack8(pk, o);  // sum what was stored (bf16-rounded), as ln_bwd_kernel and the GEMM colsum do
+#pragma unroll
+                for (int q = 0; q < 8; ++q) dxs[v][q] += o[q];
+            }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[st]);  // this warp no longer reads the stage
