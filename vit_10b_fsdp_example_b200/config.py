@@ -82,6 +82,10 @@ def build_arg_parser() -> argparse.ArgumentParser:
                         help="probability of CutMix instead of Mixup when both are on")
     parser.add_argument("--smoothing", type=_smoothing, default=0.0,
                         help="label smoothing of the (mixed) training targets; 0 = off")
+    parser.add_argument("--qk_norm", action="store_true",
+                        help="QK normalisation (timm Attention(qk_norm=True), ViT-22B): a LayerNorm over the head dim "
+                             "of every query and key head before the attention scores, with learned weight and bias "
+                             "per block; keeps the attention logits bounded at large scale")
     return parser
 
 
@@ -139,6 +143,7 @@ class ViTConfig:
     mixup_prob: float = 1.0  # probability that a step mixes
     mixup_switch_prob: float = 0.5  # probability of CutMix when both are on
     smoothing: float = 0.0  # label smoothing of the training targets
+    qk_norm: bool = False  # per-head LayerNorm on q and k (timm Attention(qk_norm=True))
 
     def __post_init__(self):
         if not 0.0 <= self.drop_path_rate < 1.0:
@@ -166,7 +171,7 @@ class ViTConfig:
                    num_classes=cfg.num_classes, drop_path_rate=getattr(cfg, "drop_path_rate", 0.0),
                    mixup=getattr(cfg, "mixup", 0.0), cutmix=getattr(cfg, "cutmix", 0.0),
                    mixup_prob=getattr(cfg, "mixup_prob", 1.0), mixup_switch_prob=getattr(cfg, "mixup_switch_prob", 0.5),
-                   smoothing=getattr(cfg, "smoothing", 0.0))
+                   smoothing=getattr(cfg, "smoothing", 0.0), qk_norm=getattr(cfg, "qk_norm", False))
 
     @property
     def grid(self) -> int:
@@ -197,7 +202,8 @@ class ViTConfig:
 
     def block_numel(self) -> int:
         D, Hd = self.embed_dim, self.hidden_dim
-        return 2 * D + (3 * D * D + 3 * D) + (D * D + D) + 2 * D + (Hd * D + Hd) + (D * Hd + D)
+        qk = 4 * self.head_dim if self.qk_norm else 0  # q_norm / k_norm weight and bias
+        return 2 * D + (3 * D * D + 3 * D) + qk + (D * D + D) + 2 * D + (Hd * D + Hd) + (D * Hd + D)
 
     def root_numel(self) -> int:
         D = self.embed_dim

@@ -204,6 +204,39 @@ void dgelu_mul(Tensor dg, Tensor u, Tensor du) {
     b200::dgelu_mul(bf16_ptr(dg), bf16_ptr(u), bf16_mut(du), u.numel(), cur_stream());
 }
 
+// qkv / out: [T, >= 3 H hd] row-major bf16 (out may be qkv: in place); mean / rstd: fp32 [T * 2 * H].
+void qk_norm_fwd(Tensor qkv, Tensor wq, Tensor bq, Tensor wk, Tensor bk, Tensor out, Tensor mean, Tensor rstd,
+                 int64_t H, int64_t hd, double eps) {
+    c10::cuda::CUDAGuard guard(qkv.device());
+    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && out.dim() == 2 && out.stride(1) == 1 &&
+                    out.size(0) == qkv.size(0), "qk_norm_fwd: qkv and out must be row-major [T, 3D] matrices");
+    const int64_t T = qkv.size(0);
+    for (const Tensor* w : {&wq, &bq, &wk, &bk})
+        TORCH_CHECK(w->is_contiguous() && w->numel() == hd, "qk_norm_fwd: weights and biases must be contiguous [hd]");
+    TORCH_CHECK(mean.is_contiguous() && rstd.is_contiguous() && mean.numel() == T * 2 * H && rstd.numel() == T * 2 * H,
+                "qk_norm_fwd: mean / rstd must be contiguous [T * 2 * H]");
+    b200::qk_norm_fwd(bf16_ptr(qkv), qkv.stride(0), bf16_ptr(wq), bf16_ptr(bq), bf16_ptr(wk), bf16_ptr(bk),
+                      bf16_mut(out), out.stride(0), f32_ptr(mean), f32_ptr(rstd), (int)T, (int)H, (int)hd, (float)eps,
+                      cur_stream());
+}
+void qk_norm_bwd(Tensor dqkv, Tensor qkv, Tensor wq, Tensor wk, Tensor mean, Tensor rstd, Tensor dwq, Tensor dbq,
+                 Tensor dwk, Tensor dbk, Tensor colsum, int64_t H, int64_t hd) {
+    c10::cuda::CUDAGuard guard(qkv.device());
+    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && dqkv.dim() == 2 && dqkv.stride(1) == 1 &&
+                    dqkv.size(0) == qkv.size(0), "qk_norm_bwd: qkv and dqkv must be row-major [T, 3D] matrices");
+    const int64_t T = qkv.size(0);
+    TORCH_CHECK(wq.is_contiguous() && wk.is_contiguous() && wq.numel() == hd && wk.numel() == hd,
+                "qk_norm_bwd: weights must be contiguous [hd]");
+    TORCH_CHECK(mean.is_contiguous() && rstd.is_contiguous() && mean.numel() == T * 2 * H && rstd.numel() == T * 2 * H,
+                "qk_norm_bwd: mean / rstd must be contiguous [T * 2 * H]");
+    for (const Tensor* a : {&dwq, &dbq, &dwk, &dbk})
+        TORCH_CHECK(a->is_contiguous() && a->numel() == hd, "qk_norm_bwd: dw / db must be contiguous fp32 [hd]");
+    TORCH_CHECK(colsum.is_contiguous() && colsum.numel() >= 2 * H * hd, "qk_norm_bwd: colsum must be fp32 [>= 2 H hd]");
+    b200::qk_norm_bwd(bf16_mut(dqkv), dqkv.stride(0), bf16_ptr(qkv), qkv.stride(0), bf16_ptr(wq), bf16_ptr(wk),
+                      f32_ptr(mean), f32_ptr(rstd), f32_ptr(dwq), f32_ptr(dbq), f32_ptr(dwk), f32_ptr(dbk),
+                      f32_ptr(colsum), (int)T, (int)H, (int)hd, cur_stream());
+}
+
 void colsum(Tensor x, Tensor out) {
     c10::cuda::CUDAGuard guard(x.device());
     const int C = (int)x.size(-1);
@@ -375,6 +408,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("drop_path_bwd", &drop_path_bwd);
     m.def("meanpool_fwd", &meanpool_fwd);
     m.def("meanpool_bwd", &meanpool_bwd);
+    m.def("qk_norm_fwd", &qk_norm_fwd);
+    m.def("qk_norm_bwd", &qk_norm_bwd);
     m.def("colsum", &colsum);
     m.def("sumsq", &sumsq);
     m.def("adamw_split", &adamw_split);

@@ -54,6 +54,19 @@ void drop_path_bwd(const __nv_bfloat16* dy, const float* scale, __nv_bfloat16* d
 void meanpool_fwd(const __nv_bfloat16* xn, __nv_bfloat16* pooled, int B, int N, int D, cudaStream_t stream);
 void meanpool_bwd(const __nv_bfloat16* dpooled, __nv_bfloat16* dxn, int B, int N, int D, cudaStream_t stream);
 void colsum(const __nv_bfloat16* x, float* out, int64_t rows, int C, cudaStream_t stream);
+
+// QK normalisation (qk_norm.cu) on the packed [T, 3D] qkv buffer, D = H * hd, hd % 8 == 0 and 8 <= hd <= 256.
+// Forward: out[:, 0:2D) = LayerNorm over hd of each q head (wq, bq) and k head (wk, bk); mean / rstd fp32 [T, 2, H].
+// out == qkv (ld_out == ld) works in place and leaves the v columns alone; a separate out gets a copy of them.
+void qk_norm_fwd(const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* wq, const __nv_bfloat16* bq,
+                 const __nv_bfloat16* wk, const __nv_bfloat16* bk, __nv_bfloat16* out, int64_t ld_out, float* mean,
+                 float* rstd, int T, int H, int hd, float eps, cudaStream_t stream);
+// Backward, in place on dqkv[:, 0:2D) (the gradient of the normalised q / k in, of the un-normalised q / k out; the dv
+// columns are not touched).  dwq / dbq / dwk / dbk fp32 [hd] and colsum fp32 [2D] (column sums of the new bf16 dq / dk)
+// are atomically added to: zero them first.
+void qk_norm_bwd(__nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* wq,
+                 const __nv_bfloat16* wk, const float* mean, const float* rstd, float* dwq, float* dbq, float* dwk,
+                 float* dbk, float* colsum, int T, int H, int hd, cudaStream_t stream);
 void sumsq(const void* x, bool is_bf16, int64_t n, float* out, cudaStream_t stream);
 
 // hyper (optional, device): [lr, step] override the host values (CUDA-graph friendly)

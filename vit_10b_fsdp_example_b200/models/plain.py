@@ -4,7 +4,8 @@ This is the consumer side of the checkpoint contract: the reference's per-rank f
 can rebuild a full ``state_dict`` "loadable into a plain (non-FSDP) ViT" (utils.py:27-28).
 ``PlainViT.load_state_dict(consolidated, strict=True)`` accepts exactly what ``consolidate_sharded_ckpts`` writes.
 The architecture is the reference's FSDPViTModel (run_vit_training.py:99-162) without the wrappers: conv patch embed,
-learned position embedding, pre-LN blocks (LayerNorm eps 1e-5), final LayerNorm (eps 1e-6), mean pool, linear head.
+learned position embedding, pre-LN blocks (LayerNorm eps 1e-5, optionally on q and k per head: ``cfg.qk_norm``), final
+LayerNorm (eps 1e-6), mean pool, linear head.
 It runs on stock PyTorch ops (any device) and is meant for evaluation / export / fine-tuning outside the engine.
 """
 from __future__ import annotations
@@ -17,10 +18,15 @@ from ..config import ViTConfig
 
 
 class _Attention(nn.Module):
-    def __init__(self, dim: int, num_heads: int, attn_drop: float, proj_drop: float):
+    def __init__(self, dim: int, num_heads: int, attn_drop: float, proj_drop: float, qk_norm: bool = False):
         super().__init__()
         self.num_heads = num_heads
         self.qkv = nn.Linear(dim, 3 * dim, bias=True)
+        if qk_norm:  # timm Attention(qk_norm=True): LayerNorm over the head dim of q and k
+            self.q_norm = nn.LayerNorm(dim // num_heads, eps=1e-5)
+            self.k_norm = nn.LayerNorm(dim // num_heads, eps=1e-5)
+        else:
+            self.q_norm = self.k_norm = None
         self.attn_drop = attn_drop
         self.proj = nn.Linear(dim, dim)
         self.proj_drop = nn.Dropout(proj_drop)
@@ -28,6 +34,8 @@ class _Attention(nn.Module):
     def forward(self, x):
         B, N, C = x.shape
         q, k, v = self.qkv(x).reshape(B, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
+        if self.q_norm is not None:
+            q, k = self.q_norm(q), self.k_norm(k)
         o = F.scaled_dot_product_attention(q, k, v, dropout_p=self.attn_drop if self.training else 0.0)
         return self.proj_drop(self.proj(o.transpose(1, 2).reshape(B, N, C)))
 
@@ -48,7 +56,7 @@ class _Block(nn.Module):
     def __init__(self, cfg: ViTConfig):
         super().__init__()
         self.norm1 = nn.LayerNorm(cfg.embed_dim, eps=1e-5)
-        self.attn = _Attention(cfg.embed_dim, cfg.num_heads, cfg.att_dropout, cfg.mlp_dropout)
+        self.attn = _Attention(cfg.embed_dim, cfg.num_heads, cfg.att_dropout, cfg.mlp_dropout, cfg.qk_norm)
         self.norm2 = nn.LayerNorm(cfg.embed_dim, eps=1e-5)
         self.mlp = _Mlp(cfg.embed_dim, cfg.hidden_dim, cfg.mlp_dropout)
 

@@ -4,6 +4,8 @@ Architecture parity with the reference model (run_vit_training.py:99-162, timm 0
   * PatchEmbed = Conv2d(3, D, k=s=P) -> tokens; learned pos_embed; dropout           (:124-129,156-157)
   * num_blocks pre-LN blocks: x += proj(attn(norm1(x))); x += fc2(gelu(fc1(norm2(x))))  (:133-141)
     - LayerNorm eps 1e-5 inside blocks, qkv_bias=True, exact (erf) GELU
+    - optional QK normalisation (timm Attention(qk_norm=True), off in the reference): q and k of every head go through
+      LayerNorm(head_dim, eps 1e-5) (attn.q_norm / attn.k_norm, one weight and bias shared by the heads) before q k^T
     - optional stochastic depth (timm drop_path, off in the reference): x += drop_path(branch) for both branches,
       one Bernoulli per sample and branch, kept samples scaled by 1 / keep_prob, block i at rate
       linspace(0, drop_path_rate, num_blocks)[i], nothing dropped in eval
@@ -36,10 +38,13 @@ FINAL_LN_EPS = 1e-6  # run_vit_training.py:151
 # Parameter inventory
 # ------------------------------------------------------------------------------------------------
 def block_param_specs(cfg: ViTConfig) -> List[Tuple[str, Tuple[int, ...]]]:
-    D, Hd = cfg.embed_dim, cfg.hidden_dim
+    D, Hd, hd = cfg.embed_dim, cfg.hidden_dim, cfg.head_dim
+    qk = [("attn.q_norm.weight", (hd,)), ("attn.q_norm.bias", (hd,)),
+          ("attn.k_norm.weight", (hd,)), ("attn.k_norm.bias", (hd,))] if cfg.qk_norm else []
     return [
         ("norm1.weight", (D,)), ("norm1.bias", (D,)),
         ("attn.qkv.weight", (3 * D, D)), ("attn.qkv.bias", (3 * D,)),
+        *qk,  # timm's state_dict order
         ("attn.proj.weight", (D, D)), ("attn.proj.bias", (D,)),
         ("norm2.weight", (D,)), ("norm2.bias", (D,)),
         ("mlp.fc1.weight", (Hd, D)), ("mlp.fc1.bias", (Hd,)),
@@ -85,6 +90,10 @@ def init_block_params(cfg: ViTConfig, gen, device="cpu") -> Dict[str, torch.Tens
     p["attn.proj.weight"], p["attn.proj.bias"] = _linear_init(D, D, gen, device=device)
     p["mlp.fc1.weight"], p["mlp.fc1.bias"] = _linear_init(Hd, D, gen, device=device)
     p["mlp.fc2.weight"], p["mlp.fc2.bias"] = _linear_init(D, Hd, gen, device=device)
+    if cfg.qk_norm:  # nn.LayerNorm init: draws nothing, so every other parameter equals the same-seed model's
+        hd = cfg.head_dim
+        for n in ("q_norm", "k_norm"):
+            p[f"attn.{n}.weight"], p[f"attn.{n}.bias"] = torch.ones(hd, device=device), torch.zeros(hd, device=device)
     return p
 
 
@@ -184,7 +193,10 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     only what a GEMM would have to recompute (x, qkv, attention output, x1, fc1 pre-activation: 10 [T, D] units
     instead of ~17.6) and block_backward re-materialises h1 / P / h2 / gelu(u) with memory-bound kernels.
     save may also be a set of extras to keep on top of the lean set: "P" (attention probabilities),
-    "h" (both LayerNorm outputs), "g" (gelu(u)); True == all three."""
+    "h" (both LayerNorm outputs), "g" (gelu(u)); True == all three.
+    With cfg.qk_norm the attention runs on qkn = qk_norm(qkv).  The lean set keeps the un-normalised qkv and the norm's
+    fp32 statistics; save=True also keeps qkn (a checkpoint recompute goes straight into the backward, which needs it).
+    A forward that saves nothing normalises in place."""
     do_save = save is not False and save is not None
     if save is True:
         extras = frozenset(("P", "h", "g"))
@@ -209,23 +221,26 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     ag = getattr(p, "ag", None) or {}  # weights whose all-gather is fused into the GEMM that consumes them
     h1, m1, r1 = ops.ln_fwd(x, p["norm1.weight"], p["norm1.bias"], BLOCK_LN_EPS)
     qkv = ops.linear_fwd(h1, p["attn.qkv.weight"], p["attn.qkv.bias"], ag=ag.get("attn.qkv.weight"))
+    qkn = qkv  # what the attention reads: qkv, or with QK normalisation its normalised copy
+    if cfg.qk_norm:
+        qkn, qk_mean, qk_rstd = _qk_norm(ops, cfg, p, qkv, inplace=not do_save)
     masks = {}  # site name -> dropout key (the masks themselves are regenerated, never stored)
     lse = None
     if use_drop and pa > 0:
         masks["att"] = drop.key(site + 0)
         if ops.use_flash(N, hd):  # the fused kernels apply the dropout mask in registers
             if do_save:
-                a, lse = ops.attention_fwd_lse(qkv, B, N, H, hd, drop=(pa, masks["att"]))
+                a, lse = ops.attention_fwd_lse(qkn, B, N, H, hd, drop=(pa, masks["att"]))
                 P = None
             else:
-                a, P = ops.attention_fwd(qkv, B, N, H, hd, drop=(pa, masks["att"]), need_p=False)
+                a, P = ops.attention_fwd(qkn, B, N, H, hd, drop=(pa, masks["att"]), need_p=False)
         else:
-            a, P = ops.attention_fwd(qkv, B, N, H, hd, drop=(pa, masks["att"]))
+            a, P = ops.attention_fwd(qkn, B, N, H, hd, drop=(pa, masks["att"]))
     elif do_save and ops.use_flash(N, hd):
-        a, lse = ops.attention_fwd_lse(qkv, B, N, H, hd)  # backward rebuilds P from the row log-sum-exp
+        a, lse = ops.attention_fwd_lse(qkn, B, N, H, hd)  # backward rebuilds P from the row log-sum-exp
         P = None
     else:
-        a, P = ops.attention_fwd(qkv, B, N, H, hd, need_p="P" in extras)
+        a, P = ops.attention_fwd(qkn, B, N, H, hd, need_p="P" in extras)
     if use_drop and pm > 0:
         # timm feeds `drop` to both proj_drop and the two MLP dropouts
         masks["proj"] = drop.key(site + 1)
@@ -252,6 +267,10 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     saved = dict(x=x, m1=m1, r1=r1, qkv=qkv, a=a, x1=x1, m2=m2, r2=r2, u=u, masks=masks, lse=lse)
     if dpath is not None:
         saved["dpath"] = dpath
+    if cfg.qk_norm:
+        saved["qk_mean"], saved["qk_rstd"] = qk_mean, qk_rstd
+        if save is True:
+            saved["qkn"] = qkn
     if "P" in extras and lse is None:
         saved["P"] = P
     if "h" in extras:
@@ -321,18 +340,34 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
         G["attn.proj.bias"].copy_(dx1_sum)
     ops.linear_wgrad(dt, s["a"], out=G["attn.proj.weight"])
     da = ops.linear_dgrad(dt, p["attn.proj.weight"])
+    qkn = s["qkv"]
+    if cfg.qk_norm:
+        qkn = s.pop("qkn", None)
+        if qkn is None:  # not kept: rebuild the normalised copy the attention read
+            qkn = _qk_norm(ops, cfg, p, s["qkv"], inplace=False)[0]
     if s.get("lse") is not None:  # flash-style: P (and the dropout mask) is rebuilt inside the fused backward kernels
-        dqkv, dbqkv = ops.attention_bwd_lse(da, s["qkv"], s["a"], s["lse"], B, N, H, hd, want_colsum=True,
+        dqkv, dbqkv = ops.attention_bwd_lse(da, qkn, s["a"], s["lse"], B, N, H, hd, want_colsum=True,
                                             drop=(pa, masks["att"]) if "att" in masks else None)
     else:
         if s.get("P") is None:
-            s["P"] = ops.attention_probs(s["qkv"], B, N, H, hd)
+            s["P"] = ops.attention_probs(qkn, B, N, H, hd)
         if "att" in masks:
-            dqkv, dbqkv = ops.attention_bwd(da, s["qkv"], s["P"], B, N, H, hd, want_colsum=True,
+            dqkv, dbqkv = ops.attention_bwd(da, qkn, s["P"], B, N, H, hd, want_colsum=True,
                                             drop=(pa, masks["att"]))
         else:
-            dqkv, dbqkv = ops.attention_bwd(da, s["qkv"], s["P"], B, N, H, hd, want_colsum=True)
-    del da
+            dqkv, dbqkv = ops.attention_bwd(da, qkn, s["P"], B, N, H, hd, want_colsum=True)
+    del da, qkn
+    if cfg.qk_norm:
+        # dq / dk become the gradients of the un-normalised q / k; the bias is added before the norm, so the column
+        # sums of the new dq / dk are the q / k part of the qkv bias gradient (dv and its sums are unchanged)
+        D = cfg.embed_dim
+        _, dwq, dbq, dwk, dbk, cs = ops.qk_norm_bwd(dqkv, s["qkv"], H, hd, p["attn.q_norm.weight"],
+                                                    p["attn.k_norm.weight"], s["qk_mean"], s["qk_rstd"])
+        dbqkv[: 2 * D].copy_(cs)
+        G["attn.q_norm.weight"].copy_(dwq)
+        G["attn.q_norm.bias"].copy_(dbq)
+        G["attn.k_norm.weight"].copy_(dwk)
+        G["attn.k_norm.bias"].copy_(dbk)
     G["attn.qkv.bias"].copy_(dbqkv)
     s["P"] = None
     h1 = s.pop("h1", None)
@@ -346,6 +381,11 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     G["norm1.weight"].copy_(dn1w)
     G["norm1.bias"].copy_(dn1b)
     return dx, dx_sum
+
+
+def _qk_norm(ops, cfg: ViTConfig, p, qkv, inplace: bool):
+    return ops.qk_norm_fwd(qkv, cfg.num_heads, cfg.head_dim, p["attn.q_norm.weight"], p["attn.q_norm.bias"],
+                           p["attn.k_norm.weight"], p["attn.k_norm.bias"], BLOCK_LN_EPS, inplace=inplace)
 
 
 # ------------------------------------------------------------------------------------------------

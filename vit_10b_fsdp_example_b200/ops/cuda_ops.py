@@ -9,6 +9,8 @@ Every function launches hand-written kernels from ``_C.so``:
     (the kernels regenerate the Philox mask of ``dropout`` in registers).  The un-fused path (batched wgmma GEMMs +
     softmax / softmax-backward kernels with materialised P) remains for B200_FUSED_ATTN_BWD=0 and unsupported shapes.
   * LayerNorm fwd/bwd, cross-entropy, im2col, column sums, sum of squares, fused AdamW.
+  * QK normalisation: per-head LayerNorm of q and k on the packed qkv buffer and its backward (``qk_norm_fwd`` /
+    ``qk_norm_bwd``, csrc/qk_norm.cu).
   * stochastic depth: per-sample Philox scales (``drop_path_scale``), applied as a row scale in the proj / fc2 GEMM
     epilogues, and ``drop_path_bwd`` (scaled branch gradient + its bias gradient in one pass).
 
@@ -144,6 +146,30 @@ def ln_bwd(dy, x, w, mean, rstd, dres=None, want_dxsum: bool = False):
     acc = torch.zeros(3 if want_dxsum else 2, D, dtype=torch.float32, device=x.device)
     _C.layernorm_bwd(dy, x, w, mean, rstd, dres, dx, acc[0], acc[1], acc[2] if want_dxsum else None)
     return dx, acc[0], acc[1], (acc[2] if want_dxsum else None)
+
+
+# ------------------------------------------------------------------------------------------------
+# QK normalisation (csrc/qk_norm.cu): per-head LayerNorm of q and k on the packed qkv buffer
+# ------------------------------------------------------------------------------------------------
+def qk_norm_fwd(qkv, H: int, hd: int, wq, bq, wk, bk, eps: float, inplace: bool = False):
+    """Returns (out, mean, rstd): out = qkv with every q head normalised over hd (weight wq, bias bq) and every k head
+    (wk, bk), v unchanged; mean / rstd fp32 [T * 2 * H].  inplace=True writes into qkv itself (the v columns are not
+    touched) and returns it; otherwise out is a new [T, 3D] buffer that also receives a copy of v."""
+    T = qkv.shape[0]
+    out = qkv if inplace else torch.empty(T, 3 * H * hd, dtype=qkv.dtype, device=qkv.device)
+    mean = torch.empty(T * 2 * H, dtype=torch.float32, device=qkv.device)
+    rstd = torch.empty(T * 2 * H, dtype=torch.float32, device=qkv.device)
+    _C.qk_norm_fwd(qkv, wq, bq, wk, bk, out, mean, rstd, H, hd, float(eps))
+    return out, mean, rstd
+
+
+def qk_norm_bwd(dqkv, qkv, H: int, hd: int, wq, wk, mean, rstd):
+    """In place on dqkv[:, 0:2D); returns (dqkv, dwq, dbq, dwk, dbk, colsum[2D]) like ``torch_ops.qk_norm_bwd``."""
+    acc = torch.zeros(4 * hd + 2 * H * hd, dtype=torch.float32, device=qkv.device)
+    dwq, dbq, dwk, dbk = acc[:4 * hd].view(4, hd)
+    cs = acc[4 * hd:]
+    _C.qk_norm_bwd(dqkv, qkv, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, cs, H, hd)
+    return dqkv, dwq, dbq, dwk, dbk, cs
 
 
 # ------------------------------------------------------------------------------------------------

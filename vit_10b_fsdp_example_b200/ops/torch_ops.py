@@ -52,6 +52,44 @@ def ln_bwd(dy, x, w, mean, rstd, dres=None, want_dxsum: bool = False):
 
 
 # ------------------------------------------------------------------------------------------------
+# QK normalisation (timm Attention(qk_norm=True): q_norm / k_norm = nn.LayerNorm(head_dim) applied per head)
+# qkv is the packed [T, 3D] projection (D = H * hd); statistics are indexed [T, 2, H] (q heads, then k heads).
+# ------------------------------------------------------------------------------------------------
+def qk_norm_fwd(qkv, H: int, hd: int, wq, bq, wk, bk, eps: float, inplace: bool = False):
+    """Returns (out, mean, rstd): out = qkv with every q head normalised over hd (weight wq, bias bq) and every k head
+    (wk, bk), v unchanged; mean / rstd fp32 [T * 2 * H].  inplace=True writes into qkv itself and returns it."""
+    T, D = qkv.shape[0], H * hd
+    x = _f32(qkv[:, : 2 * D]).reshape(T, 2, H, hd)
+    mean = x.mean(dim=-1)
+    rstd = torch.rsqrt(x.var(dim=-1, unbiased=False) + eps)
+    w = torch.stack([_f32(wq), _f32(wk)])[None, :, None, :]
+    b = torch.stack([_f32(bq), _f32(bk)])[None, :, None, :]
+    y = ((x - mean[..., None]) * rstd[..., None] * w + b).reshape(T, 2 * D).to(qkv.dtype)
+    out = qkv if inplace else qkv.clone()
+    out[:, : 2 * D] = y
+    return out, mean.reshape(-1), rstd.reshape(-1)
+
+
+def qk_norm_bwd(dqkv, qkv, H: int, hd: int, wq, wk, mean, rstd):
+    """LayerNorm backward of the q / k heads, in place on dqkv[:, 0:2D) (gradient of the normalised q / k in, of the
+    un-normalised q / k out; dv untouched).  Returns (dqkv, dwq, dbq, dwk, dbk, colsum): fp32 [hd] parameter
+    gradients summed over all T * H heads of each side, and fp32 [2D] column sums of the new (rounded) dq / dk, which
+    are the q / k part of the qkv bias gradient."""
+    T, D = qkv.shape[0], H * hd
+    x = _f32(qkv[:, : 2 * D]).reshape(T, 2, H, hd)
+    dy = _f32(dqkv[:, : 2 * D]).reshape(T, 2, H, hd)
+    m, r = mean.view(T, 2, H, 1), rstd.view(T, 2, H, 1)
+    xhat = (x - m) * r
+    g = dy * torch.stack([_f32(wq), _f32(wk)])[None, :, None, :]
+    dx = r * (g - g.mean(dim=-1, keepdim=True) - xhat * (g * xhat).mean(dim=-1, keepdim=True))
+    dw = (dy * xhat).sum(dim=(0, 2))
+    db = dy.sum(dim=(0, 2))
+    dqkv[:, : 2 * D] = dx.reshape(T, 2 * D).to(dqkv.dtype)
+    cs = _f32(dqkv[:, : 2 * D]).sum(dim=0)
+    return dqkv, dw[0], db[0], dw[1], db[1], cs
+
+
+# ------------------------------------------------------------------------------------------------
 # Linear layers (timm Attention.qkv / proj, Mlp.fc1 / fc2, head) and their backward
 # ------------------------------------------------------------------------------------------------
 def gelu(x):
