@@ -86,6 +86,10 @@ def build_arg_parser() -> argparse.ArgumentParser:
                         help="QK normalisation (timm Attention(qk_norm=True), ViT-22B): a LayerNorm over the head dim "
                              "of every query and key head before the attention scores, with learned weight and bias "
                              "per block; keeps the attention logits bounded at large scale")
+    parser.add_argument("--init_values", type=_non_negative("--init_values"), default=0.0,
+                        help="LayerScale (CaiT, timm VisionTransformer(init_values=...)): every block scales its "
+                             "attention and MLP branches by learned per-channel vectors ls1.gamma / ls2.gamma that "
+                             "start at this value (1e-5 to 1e-4 in DeiT III / DINOv2 recipes); 0 = off")
     return parser
 
 
@@ -144,6 +148,7 @@ class ViTConfig:
     mixup_switch_prob: float = 0.5  # probability of CutMix when both are on
     smoothing: float = 0.0  # label smoothing of the training targets
     qk_norm: bool = False  # per-head LayerNorm on q and k (timm Attention(qk_norm=True))
+    init_values: float = 0.0  # LayerScale initial value (timm VisionTransformer(init_values=...)); 0 = off
 
     def __post_init__(self):
         if not 0.0 <= self.drop_path_rate < 1.0:
@@ -157,6 +162,8 @@ class ViTConfig:
                 raise ValueError(f"{name} must be in [0, 1], got {getattr(self, name)}")
         if not 0.0 <= self.smoothing < 1.0:
             raise ValueError(f"smoothing must be in [0, 1), got {self.smoothing}")
+        if not (self.init_values >= 0.0 and self.init_values != float("inf")):
+            raise ValueError(f"init_values must be a finite number >= 0, got {self.init_values}")
 
     @property
     def mixing(self) -> bool:
@@ -171,7 +178,8 @@ class ViTConfig:
                    num_classes=cfg.num_classes, drop_path_rate=getattr(cfg, "drop_path_rate", 0.0),
                    mixup=getattr(cfg, "mixup", 0.0), cutmix=getattr(cfg, "cutmix", 0.0),
                    mixup_prob=getattr(cfg, "mixup_prob", 1.0), mixup_switch_prob=getattr(cfg, "mixup_switch_prob", 0.5),
-                   smoothing=getattr(cfg, "smoothing", 0.0), qk_norm=getattr(cfg, "qk_norm", False))
+                   smoothing=getattr(cfg, "smoothing", 0.0), qk_norm=getattr(cfg, "qk_norm", False),
+                   init_values=getattr(cfg, "init_values", 0.0))
 
     @property
     def grid(self) -> int:
@@ -203,7 +211,8 @@ class ViTConfig:
     def block_numel(self) -> int:
         D, Hd = self.embed_dim, self.hidden_dim
         qk = 4 * self.head_dim if self.qk_norm else 0  # q_norm / k_norm weight and bias
-        return 2 * D + (3 * D * D + 3 * D) + qk + (D * D + D) + 2 * D + (Hd * D + Hd) + (D * Hd + D)
+        ls = 2 * D if self.init_values else 0  # ls1.gamma / ls2.gamma
+        return 2 * D + (3 * D * D + 3 * D) + qk + (D * D + D) + 2 * D + (Hd * D + Hd) + (D * Hd + D) + ls
 
     def root_numel(self) -> int:
         D = self.embed_dim

@@ -12,6 +12,7 @@
 #include "comm.h"
 #include "elementwise.h"
 #include "gemm_sm90.h"
+#include "layer_scale.h"
 
 namespace {
 
@@ -237,6 +238,37 @@ void qk_norm_bwd(Tensor dqkv, Tensor qkv, Tensor wq, Tensor wk, Tensor mean, Ten
                       f32_ptr(colsum), (int)T, (int)H, (int)hd, cur_stream());
 }
 
+// LayerScale folded into a linear layer.  W / dW / Wg: contiguous bf16 [D, K]; b / gamma / bg: contiguous bf16 [D];
+// S / db / dgamma: contiguous fp32 [D].
+void check_layer_scale(const char* what, const Tensor& W, const Tensor& b, const Tensor& gamma, const Tensor& Wg) {
+    TORCH_CHECK(W.is_cuda() && W.scalar_type() == at::kBFloat16 && W.dim() == 2 && W.is_contiguous(), what,
+                ": W must be a contiguous bf16 CUDA [D, K] matrix");
+    TORCH_CHECK(Wg.scalar_type() == at::kBFloat16 && Wg.is_contiguous() && Wg.sizes() == W.sizes(), what,
+                ": Wg must be a contiguous bf16 matrix of W's shape");
+    for (const Tensor* t : {&b, &gamma})
+        TORCH_CHECK(t->scalar_type() == at::kBFloat16 && t->is_contiguous() && t->numel() == W.size(0), what,
+                    ": b and gamma must be contiguous bf16 vectors of length D = W.size(0)");
+}
+void layer_scale_fold(Tensor W, Tensor b, Tensor gamma, Tensor Wg, Tensor bg) {
+    c10::cuda::CUDAGuard guard(W.device());
+    check_layer_scale("layer_scale_fold", W, b, gamma, Wg);
+    TORCH_CHECK(bg.scalar_type() == at::kBFloat16 && bg.is_contiguous() && bg.numel() == W.size(0),
+                "layer_scale_fold: bg must be a contiguous bf16 vector of length D = W.size(0)");
+    b200::layer_scale_fold(bf16_ptr(W), bf16_ptr(b), bf16_ptr(gamma), bf16_mut(Wg), bf16_mut(bg), W.size(0), W.size(1),
+                           cur_stream());
+}
+void layer_scale_bwd(Tensor W, Tensor b, Tensor gamma, Tensor dW, Tensor S, Tensor Wg, Tensor db, Tensor dgamma) {
+    c10::cuda::CUDAGuard guard(W.device());
+    check_layer_scale("layer_scale_bwd", W, b, gamma, Wg);
+    TORCH_CHECK(dW.scalar_type() == at::kBFloat16 && dW.is_contiguous() && dW.sizes() == W.sizes(),
+                "layer_scale_bwd: dW must be a contiguous bf16 matrix of W's shape");
+    for (const Tensor* t : {&S, &db, &dgamma})
+        TORCH_CHECK(t->scalar_type() == at::kFloat && t->is_contiguous() && t->numel() == W.size(0),
+                    "layer_scale_bwd: S, db and dgamma must be contiguous fp32 vectors of length D = W.size(0)");
+    b200::layer_scale_bwd(bf16_ptr(W), bf16_ptr(b), bf16_ptr(gamma), bf16_mut(dW), f32_ptr(S), bf16_mut(Wg),
+                          f32_ptr(db), f32_ptr(dgamma), W.size(0), W.size(1), cur_stream());
+}
+
 void colsum(Tensor x, Tensor out) {
     c10::cuda::CUDAGuard guard(x.device());
     const int C = (int)x.size(-1);
@@ -410,6 +442,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("meanpool_bwd", &meanpool_bwd);
     m.def("qk_norm_fwd", &qk_norm_fwd);
     m.def("qk_norm_bwd", &qk_norm_bwd);
+    m.def("layer_scale_fold", &layer_scale_fold);
+    m.def("layer_scale_bwd", &layer_scale_bwd);
     m.def("colsum", &colsum);
     m.def("sumsq", &sumsq);
     m.def("adamw_split", &adamw_split);

@@ -4,8 +4,8 @@ This is the consumer side of the checkpoint contract: the reference's per-rank f
 can rebuild a full ``state_dict`` "loadable into a plain (non-FSDP) ViT" (utils.py:27-28).
 ``PlainViT.load_state_dict(consolidated, strict=True)`` accepts exactly what ``consolidate_sharded_ckpts`` writes.
 The architecture is the reference's FSDPViTModel (run_vit_training.py:99-162) without the wrappers: conv patch embed,
-learned position embedding, pre-LN blocks (LayerNorm eps 1e-5, optionally on q and k per head: ``cfg.qk_norm``), final
-LayerNorm (eps 1e-6), mean pool, linear head.
+learned position embedding, pre-LN blocks (LayerNorm eps 1e-5, optionally on q and k per head: ``cfg.qk_norm``;
+optionally LayerScale on both branches: ``cfg.init_values``), final LayerNorm (eps 1e-6), mean pool, linear head.
 It runs on stock PyTorch ops (any device) and is meant for evaluation / export / fine-tuning outside the engine.
 """
 from __future__ import annotations
@@ -52,17 +52,30 @@ class _Mlp(nn.Module):
         return self.drop(self.fc2(self.drop(self.act(self.fc1(x)))))
 
 
+class _LayerScale(nn.Module):
+    """timm LayerScale: x * gamma, gamma [dim] starting at init_values."""
+
+    def __init__(self, dim: int, init_values: float):
+        super().__init__()
+        self.gamma = nn.Parameter(init_values * torch.ones(dim))
+
+    def forward(self, x):
+        return x * self.gamma
+
+
 class _Block(nn.Module):
     def __init__(self, cfg: ViTConfig):
         super().__init__()
         self.norm1 = nn.LayerNorm(cfg.embed_dim, eps=1e-5)
         self.attn = _Attention(cfg.embed_dim, cfg.num_heads, cfg.att_dropout, cfg.mlp_dropout, cfg.qk_norm)
+        self.ls1 = _LayerScale(cfg.embed_dim, cfg.init_values) if cfg.init_values else nn.Identity()
         self.norm2 = nn.LayerNorm(cfg.embed_dim, eps=1e-5)
         self.mlp = _Mlp(cfg.embed_dim, cfg.hidden_dim, cfg.mlp_dropout)
+        self.ls2 = _LayerScale(cfg.embed_dim, cfg.init_values) if cfg.init_values else nn.Identity()
 
     def forward(self, x):
-        x = x + self.attn(self.norm1(x))
-        return x + self.mlp(self.norm2(x))
+        x = x + self.ls1(self.attn(self.norm1(x)))
+        return x + self.ls2(self.mlp(self.norm2(x)))
 
 
 class _PatchEmbed(nn.Module):

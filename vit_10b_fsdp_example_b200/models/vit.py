@@ -9,6 +9,11 @@ Architecture parity with the reference model (run_vit_training.py:99-162, timm 0
     - optional stochastic depth (timm drop_path, off in the reference): x += drop_path(branch) for both branches,
       one Bernoulli per sample and branch, kept samples scaled by 1 / keep_prob, block i at rate
       linspace(0, drop_path_rate, num_blocks)[i], nothing dropped in eval
+    - optional LayerScale (CaiT, timm VisionTransformer(init_values=...), off in the reference):
+      x += ls1.gamma * branch and x += ls2.gamma * branch, learned per-channel [D] vectors that start at init_values, in
+      training and in eval.  The scale is folded into the branch's last layer, gamma o (a W^T + b) = a (gamma o W)^T +
+      gamma o b, so the GEMMs run unchanged on the folded weight; the backward recovers dW, db and dgamma from the wgrad
+      of the un-scaled weight in one pass over the weight (ops.layer_scale_bwd)
   * optional Mixup / CutMix (timm Mixup, mode 'batch', off in the reference): drawn on the host per step (draw_mix),
     applied inside the patch im2col, with the mixed, smoothed target handled by the cross-entropy
   * final LayerNorm(eps=1e-6), mean-pool over tokens (no CLS token), Linear head      (:151-153,159-161)
@@ -41,14 +46,17 @@ def block_param_specs(cfg: ViTConfig) -> List[Tuple[str, Tuple[int, ...]]]:
     D, Hd, hd = cfg.embed_dim, cfg.hidden_dim, cfg.head_dim
     qk = [("attn.q_norm.weight", (hd,)), ("attn.q_norm.bias", (hd,)),
           ("attn.k_norm.weight", (hd,)), ("attn.k_norm.bias", (hd,))] if cfg.qk_norm else []
+    ls = [("ls1.gamma", (D,)), ("ls2.gamma", (D,))] if cfg.init_values else []
     return [
         ("norm1.weight", (D,)), ("norm1.bias", (D,)),
         ("attn.qkv.weight", (3 * D, D)), ("attn.qkv.bias", (3 * D,)),
         *qk,  # timm's state_dict order
         ("attn.proj.weight", (D, D)), ("attn.proj.bias", (D,)),
+        *ls[:1],  # timm's Block registers ls1 / ls2 after attn / mlp
         ("norm2.weight", (D,)), ("norm2.bias", (D,)),
         ("mlp.fc1.weight", (Hd, D)), ("mlp.fc1.bias", (Hd,)),
         ("mlp.fc2.weight", (D, Hd)), ("mlp.fc2.bias", (D,)),
+        *ls[1:],
     ]
 
 
@@ -94,6 +102,9 @@ def init_block_params(cfg: ViTConfig, gen, device="cpu") -> Dict[str, torch.Tens
         hd = cfg.head_dim
         for n in ("q_norm", "k_norm"):
             p[f"attn.{n}.weight"], p[f"attn.{n}.bias"] = torch.ones(hd, device=device), torch.zeros(hd, device=device)
+    if cfg.init_values:  # timm LayerScale: init_values * ones(D), no draws either
+        p["ls1.gamma"] = torch.full((D,), float(cfg.init_values), device=device)
+        p["ls2.gamma"] = torch.full((D,), float(cfg.init_values), device=device)
     return p
 
 
@@ -241,27 +252,31 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
         P = None
     else:
         a, P = ops.attention_fwd(qkn, B, N, H, hd, need_p="P" in extras)
+    w_proj, b_proj = _branch_layer(ops, cfg, p, "attn.proj", "ls1")
     if use_drop and pm > 0:
         # timm feeds `drop` to both proj_drop and the two MLP dropouts
         masks["proj"] = drop.key(site + 1)
-        t = ops.linear_fwd(a, p["attn.proj.weight"], p["attn.proj.bias"], **rs_att)
+        t = ops.linear_fwd(a, w_proj, b_proj, **rs_att)
         x1 = x + ops.dropout(t, pm, masks["proj"])  # the per-sample row scale commutes with the element mask
     else:
-        x1 = ops.linear_fwd(a, p["attn.proj.weight"], p["attn.proj.bias"], residual=x, **rs_att)
+        x1 = ops.linear_fwd(a, w_proj, b_proj, residual=x, **rs_att)
+    del w_proj, b_proj
     h2, m2, r2 = ops.ln_fwd(x1, p["norm2.weight"], p["norm2.bias"], BLOCK_LN_EPS)
     if do_save:
         g, u = ops.linear_fwd(h2, p["mlp.fc1.weight"], p["mlp.fc1.bias"], act="gelu", want_preact=True,
                               ag=ag.get("mlp.fc1.weight"))
     else:
         g, u = ops.linear_fwd(h2, p["mlp.fc1.weight"], p["mlp.fc1.bias"], act="gelu", ag=ag.get("mlp.fc1.weight")), None
+    w_fc2, b_fc2 = _branch_layer(ops, cfg, p, "mlp.fc2", "ls2")
     if use_drop and pm > 0:
         masks["fc1"] = drop.key(site + 2)
         masks["fc2"] = drop.key(site + 3)
         g = ops.dropout(g, pm, masks["fc1"])
-        t = ops.linear_fwd(g, p["mlp.fc2.weight"], p["mlp.fc2.bias"], **rs_mlp)
+        t = ops.linear_fwd(g, w_fc2, b_fc2, **rs_mlp)
         y = x1 + ops.dropout(t, pm, masks["fc2"])
     else:
-        y = ops.linear_fwd(g, p["mlp.fc2.weight"], p["mlp.fc2.bias"], residual=x1, **rs_mlp)
+        y = ops.linear_fwd(g, w_fc2, b_fc2, residual=x1, **rs_mlp)
+    del w_fc2, b_fc2
     if not do_save:
         return y, None
     saved = dict(x=x, m1=m1, r1=r1, qkv=qkv, a=a, x1=x1, m2=m2, r2=r2, u=u, masks=masks, lse=lse)
@@ -286,6 +301,9 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     p / G: parameter and gradient views of this unit.  dy_colsum = column sums of dy (fp32), which *is*
     the fc2 bias gradient; it is produced for free by whoever computed dy (the LN backward of the block
     above).  Returns (dx, colsum(dx)) for the block below.
+    With LayerScale the proj / fc2 bias gradient is gamma o colsum instead; the wgrad runs first, then
+    ``ops.layer_scale_bwd`` rescales its result and yields the bias and gamma gradients, and the dgrad uses the
+    folded weight.
     """
     N, H, hd = cfg.num_patches, cfg.num_heads, cfg.head_dim
     pa, pm = cfg.att_dropout, cfg.mlp_dropout
@@ -294,14 +312,15 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     # ---- MLP ----
     if dpath is not None:  # the branch gradient is scaled per sample; the residual gradient dy stays as it is
         dt = ops.dropout(dy, pm, masks["fc2"]) if "fc2" in masks else dy
-        dt, db2 = ops.drop_path_bwd(dt, dpath[1], N)
-        G["mlp.fc2.bias"].copy_(db2)
+        dt, s2 = ops.drop_path_bwd(dt, dpath[1], N)
     elif "fc2" in masks:
         dt = ops.dropout(dy, pm, masks["fc2"])
-        G["mlp.fc2.bias"].copy_(ops.colsum(dt))
+        s2 = ops.colsum(dt)
     else:
         dt = dy
-        G["mlp.fc2.bias"].copy_(dy_colsum)
+        s2 = dy_colsum
+    if not cfg.init_values:
+        G["mlp.fc2.bias"].copy_(s2)
     g = s.pop("g", None)
     if g is None:  # not kept: re-materialise from the pre-activation
         g = ops.gelu_fwd(s["u"])
@@ -309,12 +328,14 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
             g = ops.dropout(g, pm, masks["fc1"])
     ops.linear_wgrad(dt, g, out=G["mlp.fc2.weight"])
     del g
+    w_fc2 = _layer_scale_bwd(ops, p, G, "mlp.fc2", "ls2", s2) if cfg.init_values else p["mlp.fc2.weight"]
     if "fc1" in masks:
-        dg = ops.dropout(ops.linear_dgrad(dt, p["mlp.fc2.weight"]), pm, masks["fc1"])
+        dg = ops.dropout(ops.linear_dgrad(dt, w_fc2), pm, masks["fc1"])
         du = ops.dgelu_mul(dg, s["u"])
         db1 = ops.colsum(du)
     else:
-        du, db1 = ops.linear_dgrad(dt, p["mlp.fc2.weight"], dgelu_preact=s["u"], want_colsum=True)
+        du, db1 = ops.linear_dgrad(dt, w_fc2, dgelu_preact=s["u"], want_colsum=True)
+    del w_fc2
     G["mlp.fc1.bias"].copy_(db1)
     h2 = s.pop("h2", None)
     if h2 is None:
@@ -330,16 +351,19 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     # ---- attention ----
     if dpath is not None:
         dt = ops.dropout(dx1, pm, masks["proj"]) if "proj" in masks else dx1
-        dt, dbp = ops.drop_path_bwd(dt, dpath[0], N)
-        G["attn.proj.bias"].copy_(dbp)
+        dt, s1 = ops.drop_path_bwd(dt, dpath[0], N)
     elif "proj" in masks:
         dt = ops.dropout(dx1, pm, masks["proj"])
-        G["attn.proj.bias"].copy_(ops.colsum(dt))
+        s1 = ops.colsum(dt)
     else:
         dt = dx1
-        G["attn.proj.bias"].copy_(dx1_sum)
+        s1 = dx1_sum
+    if not cfg.init_values:
+        G["attn.proj.bias"].copy_(s1)
     ops.linear_wgrad(dt, s["a"], out=G["attn.proj.weight"])
-    da = ops.linear_dgrad(dt, p["attn.proj.weight"])
+    w_proj = _layer_scale_bwd(ops, p, G, "attn.proj", "ls1", s1) if cfg.init_values else p["attn.proj.weight"]
+    da = ops.linear_dgrad(dt, w_proj)
+    del w_proj
     qkn = s["qkv"]
     if cfg.qk_norm:
         qkn = s.pop("qkn", None)
@@ -381,6 +405,22 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     G["norm1.weight"].copy_(dn1w)
     G["norm1.bias"].copy_(dn1b)
     return dx, dx_sum
+
+
+def _branch_layer(ops, cfg: ViTConfig, p, layer: str, ls: str):
+    """Weight and bias of a branch's last layer, with LayerScale folded in: (gamma o W, gamma o b)."""
+    w, b = p[f"{layer}.weight"], p[f"{layer}.bias"]
+    return ops.layer_scale_fold(w, b, p[f"{ls}.gamma"]) if cfg.init_values else (w, b)
+
+
+def _layer_scale_bwd(ops, p, G, layer: str, ls: str, colsum):
+    """After the wgrad has written M = dy'^T a into G[layer.weight]: turns it into dW = gamma o M and writes the bias
+    and gamma gradients (colsum = column sums of dy').  Returns the folded weight the dgrad multiplies by."""
+    wg, db, dgamma = ops.layer_scale_bwd(p[f"{layer}.weight"], p[f"{layer}.bias"], p[f"{ls}.gamma"],
+                                         G[f"{layer}.weight"], colsum)
+    G[f"{layer}.bias"].copy_(db)
+    G[f"{ls}.gamma"].copy_(dgamma)
+    return wg
 
 
 def _qk_norm(ops, cfg: ViTConfig, p, qkv, inplace: bool):

@@ -11,6 +11,8 @@ Every function launches hand-written kernels from ``_C.so``:
   * LayerNorm fwd/bwd, cross-entropy, im2col, column sums, sum of squares, fused AdamW.
   * QK normalisation: per-head LayerNorm of q and k on the packed qkv buffer and its backward (``qk_norm_fwd`` /
     ``qk_norm_bwd``, csrc/qk_norm.cu).
+  * LayerScale: the per-channel branch scale folded into the proj / fc2 weight and bias, and its backward on the
+    weight gradient (``layer_scale_fold`` / ``layer_scale_bwd``, csrc/layer_scale.cu).
   * stochastic depth: per-sample Philox scales (``drop_path_scale``), applied as a row scale in the proj / fc2 GEMM
     epilogues, and ``drop_path_bwd`` (scaled branch gradient + its bias gradient in one pass).
 
@@ -170,6 +172,25 @@ def qk_norm_bwd(dqkv, qkv, H: int, hd: int, wq, wk, mean, rstd):
     cs = acc[4 * hd:]
     _C.qk_norm_bwd(dqkv, qkv, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, cs, H, hd)
     return dqkv, dwq, dbq, dwk, dbk, cs
+
+
+# ------------------------------------------------------------------------------------------------
+# LayerScale (csrc/layer_scale.cu): per-channel branch scale folded into the proj / fc2 weight and bias
+# ------------------------------------------------------------------------------------------------
+def layer_scale_fold(W, b, gamma):
+    """(Wg, bg) = (bf16(gamma_c * W[c, :]), bf16(gamma_c * b_c)) like ``torch_ops.layer_scale_fold``."""
+    Wg = torch.empty_like(W, memory_format=torch.contiguous_format)
+    bg = torch.empty_like(b, memory_format=torch.contiguous_format)
+    _C.layer_scale_fold(W, b, gamma, Wg, bg)
+    return Wg, bg
+
+
+def layer_scale_bwd(W, b, gamma, dW, S):
+    """In place on dW (M in, gamma o M out); returns (Wg, db, dgamma) like ``torch_ops.layer_scale_bwd``."""
+    Wg = torch.empty_like(W, memory_format=torch.contiguous_format)
+    out = torch.empty(2, W.shape[0], dtype=torch.float32, device=W.device)
+    _C.layer_scale_bwd(W, b, gamma, dW, S, Wg, out[0], out[1])
+    return Wg, out[0], out[1]
 
 
 # ------------------------------------------------------------------------------------------------

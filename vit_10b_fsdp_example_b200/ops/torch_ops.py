@@ -90,6 +90,25 @@ def qk_norm_bwd(dqkv, qkv, H: int, hd: int, wq, wk, mean, rstd):
 
 
 # ------------------------------------------------------------------------------------------------
+# LayerScale (timm LayerScale: x * gamma on a branch u = a W^T + b), folded into the layer's weight and bias
+# ------------------------------------------------------------------------------------------------
+def layer_scale_fold(W, b, gamma):
+    """(Wg, bg) = (gamma_c * W[c, :], gamma_c * b_c), each rounded once to W's dtype: a Wg^T + bg = gamma o u."""
+    g = _f32(gamma)
+    return (_f32(W) * g[:, None]).to(W.dtype), (_f32(b) * g).to(b.dtype)
+
+
+def layer_scale_bwd(W, b, gamma, dW, S):
+    """dW holds M = dy'^T a (the wgrad of the un-scaled layer) and is overwritten with gamma o M; S = fp32 colsum(dy').
+    Returns (Wg, db, dgamma): Wg as ``layer_scale_fold``, db = gamma o S and dgamma_c = sum_k W[c, k] M[c, k] + b_c S_c
+    (= sum_r dy'[r, c] u[r, c]), both fp32 [D]."""
+    g, m, s = _f32(gamma), _f32(dW), _f32(S)
+    dgamma = (_f32(W) * m).sum(dim=1) + _f32(b) * s
+    dW.copy_(m * g[:, None])
+    return (_f32(W) * g[:, None]).to(W.dtype), g * s, dgamma
+
+
+# ------------------------------------------------------------------------------------------------
 # Linear layers (timm Attention.qkv / proj, Mlp.fc1 / fc2, head) and their backward
 # ------------------------------------------------------------------------------------------------
 def gelu(x):

@@ -664,6 +664,13 @@ class FSDPViT:
         if has_qk and not self.cfg.qk_norm:
             raise ValueError("the checkpoint has attn.q_norm / attn.k_norm parameters (it was trained with QK "
                              "normalisation): pass --qk_norm to load it")
+        has_ls = any(k.endswith(("ls1.gamma", "ls2.gamma")) for k in full)
+        if self.cfg.init_values and not has_ls:
+            raise ValueError("this model uses --init_values (LayerScale), but the checkpoint has no ls1.gamma / "
+                             "ls2.gamma parameters: it was trained without LayerScale")
+        if has_ls and not self.cfg.init_values:
+            raise ValueError("the checkpoint has ls1.gamma / ls2.gamma parameters (it was trained with LayerScale): "
+                             "pass --init_values to load it (any value > 0; the learned gammas are loaded)")
         for u in self.all_units:
             lay = u.layout
             prefix = "" if u is self.root else u.name + "."
