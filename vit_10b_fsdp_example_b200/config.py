@@ -90,7 +90,26 @@ def build_arg_parser() -> argparse.ArgumentParser:
                         help="LayerScale (CaiT, timm VisionTransformer(init_values=...)): every block scales its "
                              "attention and MLP branches by learned per-channel vectors ls1.gamma / ls2.gamma that "
                              "start at this value (1e-5 to 1e-4 in DeiT III / DINOv2 recipes); 0 = off")
+    # ---- prefix tokens (timm VisionTransformer(class_token=..., reg_tokens=..., no_embed_class=...)) ----
+    parser.add_argument("--class_token", action="store_true",
+                        help="prepend a learned class token (cls_token) to every image's patch tokens and classify "
+                             "from it after the final norm (timm global_pool='token'; DeiT, DeiT III, DINOv2) instead "
+                             "of mean-pooling the patches")
+    parser.add_argument("--reg_tokens", type=_reg_tokens, default=0,
+                        help="learned register tokens placed after the class token (Darcet et al., 2023, 'Vision "
+                             "Transformers Need Registers'); needs --class_token; 0 = none")
+    parser.add_argument("--no_embed_class", action="store_true",
+                        help="pos_embed covers the patches only and the class / register tokens get no position "
+                             "embedding (timm no_embed_class=True); needs --class_token")
     return parser
+
+
+def check_prefix_flags(args) -> None:
+    """--reg_tokens and --no_embed_class only mean something next to a class token."""
+    if not args.class_token and (args.reg_tokens or args.no_embed_class):
+        flag = "--reg_tokens" if args.reg_tokens else "--no_embed_class"
+        raise ValueError(f"{flag} needs --class_token (register tokens and an un-embedded prefix exist only next to a "
+                         f"class token; mean pooling has no prefix tokens)")
 
 
 def _drop_path_rate(s: str) -> float:
@@ -118,6 +137,13 @@ def _probability(flag: str):
     return parse
 
 
+def _reg_tokens(s: str) -> int:
+    v = int(s)
+    if v < 0:
+        raise argparse.ArgumentTypeError(f"--reg_tokens must be an integer >= 0, got {s}")
+    return v
+
+
 def _smoothing(s: str) -> float:
     v = float(s)
     if not 0.0 <= v < 1.0:
@@ -126,7 +152,13 @@ def _smoothing(s: str) -> float:
 
 
 def parse_args(argv=None) -> argparse.Namespace:
-    return build_arg_parser().parse_args(argv)
+    parser = build_arg_parser()
+    args = parser.parse_args(argv)
+    try:
+        check_prefix_flags(args)
+    except ValueError as e:
+        parser.error(str(e))
+    return args
 
 
 @dataclass
@@ -149,6 +181,9 @@ class ViTConfig:
     smoothing: float = 0.0  # label smoothing of the training targets
     qk_norm: bool = False  # per-head LayerNorm on q and k (timm Attention(qk_norm=True))
     init_values: float = 0.0  # LayerScale initial value (timm VisionTransformer(init_values=...)); 0 = off
+    class_token: bool = False  # learned cls_token in front of the patches, classified from (timm global_pool='token')
+    reg_tokens: int = 0  # learned register tokens after the class token (needs class_token)
+    no_embed_class: bool = False  # pos_embed covers the patches only (timm no_embed_class=True; needs class_token)
 
     def __post_init__(self):
         if not 0.0 <= self.drop_path_rate < 1.0:
@@ -164,6 +199,9 @@ class ViTConfig:
             raise ValueError(f"smoothing must be in [0, 1), got {self.smoothing}")
         if not (self.init_values >= 0.0 and self.init_values != float("inf")):
             raise ValueError(f"init_values must be a finite number >= 0, got {self.init_values}")
+        if not (isinstance(self.reg_tokens, int) and self.reg_tokens >= 0):
+            raise ValueError(f"reg_tokens must be an integer >= 0, got {self.reg_tokens}")
+        check_prefix_flags(self)
 
     @property
     def mixing(self) -> bool:
@@ -179,7 +217,8 @@ class ViTConfig:
                    mixup=getattr(cfg, "mixup", 0.0), cutmix=getattr(cfg, "cutmix", 0.0),
                    mixup_prob=getattr(cfg, "mixup_prob", 1.0), mixup_switch_prob=getattr(cfg, "mixup_switch_prob", 0.5),
                    smoothing=getattr(cfg, "smoothing", 0.0), qk_norm=getattr(cfg, "qk_norm", False),
-                   init_values=getattr(cfg, "init_values", 0.0))
+                   init_values=getattr(cfg, "init_values", 0.0), class_token=getattr(cfg, "class_token", False),
+                   reg_tokens=getattr(cfg, "reg_tokens", 0), no_embed_class=getattr(cfg, "no_embed_class", False))
 
     @property
     def grid(self) -> int:
@@ -189,6 +228,21 @@ class ViTConfig:
     @property
     def num_patches(self) -> int:
         return self.grid * self.grid
+
+    @property
+    def num_prefix_tokens(self) -> int:
+        """P: the class token and the register tokens in front of every image's patches (0 without a class token)."""
+        return (1 + self.reg_tokens) if self.class_token else 0
+
+    @property
+    def num_tokens(self) -> int:
+        """T = N + P: the tokens per image every block runs on."""
+        return self.num_patches + self.num_prefix_tokens
+
+    @property
+    def pos_len(self) -> int:
+        """Rows of pos_embed: every token, or only the patches under no_embed_class."""
+        return self.num_patches if self.no_embed_class else self.num_tokens
 
     @property
     def head_dim(self) -> int:
@@ -216,14 +270,15 @@ class ViTConfig:
 
     def root_numel(self) -> int:
         D = self.embed_dim
-        return D * self.patch_k + D + self.num_patches * D + 2 * D + self.num_classes * D + self.num_classes
+        return (D * self.patch_k + D + self.num_prefix_tokens * D + self.pos_len * D + 2 * D + self.num_classes * D
+                + self.num_classes)
 
     def total_numel(self) -> int:
         return self.num_blocks * self.block_numel() + self.root_numel()
 
     def flops_per_image(self, grad_ckpt: bool = True) -> float:
         """Matmul FLOPs of one training step per image (fwd + bwd [+ recompute])."""
-        D, Hd, N = self.embed_dim, self.hidden_dim, self.num_patches
-        per_block = 2 * N * (3 * D * D + D * D + 2 * D * Hd) + 4 * N * N * D
+        D, Hd, N, T = self.embed_dim, self.hidden_dim, self.num_patches, self.num_tokens
+        per_block = 2 * T * (3 * D * D + D * D + 2 * D * Hd) + 4 * T * T * D
         fwd = self.num_blocks * per_block + 2 * N * self.patch_k * D + 2 * D * self.num_classes
         return fwd * (4.0 if grad_ckpt else 3.0)

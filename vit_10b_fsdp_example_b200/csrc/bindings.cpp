@@ -13,6 +13,7 @@
 #include "elementwise.h"
 #include "gemm_sm90.h"
 #include "layer_scale.h"
+#include "prefix_tokens.h"
 
 namespace {
 
@@ -269,6 +270,46 @@ void layer_scale_bwd(Tensor W, Tensor b, Tensor gamma, Tensor dW, Tensor S, Tens
                           f32_ptr(db), f32_ptr(dgamma), W.size(0), W.size(1), cur_stream());
 }
 
+// Prefix tokens (class + register tokens).  y: contiguous bf16 [B * N, D] patch rows; cls: bf16 [D]; reg: bf16
+// [R, D] or None (R = 0); pos: bf16 [P, D] (P = 1 + R) or None; x0: contiguous bf16 [B * (N + P), D].
+void check_bf16_buf(const char* what, const char* name, const Tensor& t, int64_t numel) {
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kBFloat16, what, ": ", name, " must be a bf16 CUDA tensor");
+    TORCH_CHECK(t.is_contiguous() && t.numel() == numel, what, ": ", name, " must be contiguous with ", numel,
+                " elements, got ", t.numel());
+}
+void tokens_fwd(Tensor y, Tensor cls, OptT reg, OptT pos, Tensor x0, int64_t B, int64_t N) {
+    c10::cuda::CUDAGuard guard(y.device());
+    TORCH_CHECK(y.dim() == 2, "tokens_fwd: y must be a [B * N, D] matrix");
+    const int64_t D = y.size(1);
+    TORCH_CHECK(D % 8 == 0, "tokens_fwd: need D % 8 == 0 (16-byte vectors), got D ", D);
+    check_bf16_buf("tokens_fwd", "y", y, B * N * D);
+    check_bf16_buf("tokens_fwd", "cls", cls, D);
+    int64_t P = 1;
+    if (reg.has_value()) {
+        TORCH_CHECK(reg->numel() % D == 0 && reg->numel() > 0, "tokens_fwd: reg must be [R, D] with R >= 1");
+        P += reg->numel() / D;
+        check_bf16_buf("tokens_fwd", "reg", *reg, (P - 1) * D);
+    }
+    if (pos.has_value()) check_bf16_buf("tokens_fwd", "pos", *pos, P * D);
+    check_bf16_buf("tokens_fwd", "x0", x0, B * (N + P) * D);
+    b200::tokens_fwd(bf16_ptr(y), bf16_ptr(cls), reg.has_value() ? bf16_ptr(*reg) : nullptr,
+                     pos.has_value() ? bf16_ptr(*pos) : nullptr, bf16_mut(x0), B, N, P, D, cur_stream());
+}
+// dx0: contiguous bf16 [B * (N + P), D]; dpatch: contiguous bf16 [B * N, D]; dtok: contiguous fp32 [N + P, D].
+void tokens_bwd(Tensor dx0, Tensor dpatch, Tensor dtok, int64_t B, int64_t N, int64_t P) {
+    c10::cuda::CUDAGuard guard(dx0.device());
+    TORCH_CHECK(P >= 1, "tokens_bwd: need P >= 1 prefix tokens, got P ", P);
+    TORCH_CHECK(dx0.dim() == 2, "tokens_bwd: dx0 must be a [B * (N + P), D] matrix");
+    const int64_t D = dx0.size(1);
+    TORCH_CHECK(D % 8 == 0, "tokens_bwd: need D % 8 == 0 (16-byte vectors), got D ", D);
+    check_bf16_buf("tokens_bwd", "dx0", dx0, B * (N + P) * D);
+    check_bf16_buf("tokens_bwd", "dpatch", dpatch, B * N * D);
+    TORCH_CHECK(dtok.is_cuda() && dtok.scalar_type() == at::kFloat && dtok.is_contiguous() &&
+                    dtok.numel() == (N + P) * D,
+                "tokens_bwd: dtok must be a contiguous fp32 CUDA tensor with (N + P) * D elements");
+    b200::tokens_bwd(bf16_ptr(dx0), bf16_mut(dpatch), f32_ptr(dtok), B, N, P, D, cur_stream());
+}
+
 void colsum(Tensor x, Tensor out) {
     c10::cuda::CUDAGuard guard(x.device());
     const int C = (int)x.size(-1);
@@ -444,6 +485,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("qk_norm_bwd", &qk_norm_bwd);
     m.def("layer_scale_fold", &layer_scale_fold);
     m.def("layer_scale_bwd", &layer_scale_bwd);
+    m.def("tokens_fwd", &tokens_fwd);
+    m.def("tokens_bwd", &tokens_bwd);
     m.def("colsum", &colsum);
     m.def("sumsq", &sumsq);
     m.def("adamw_split", &adamw_split);

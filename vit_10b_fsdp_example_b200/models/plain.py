@@ -6,6 +6,8 @@ can rebuild a full ``state_dict`` "loadable into a plain (non-FSDP) ViT" (utils.
 The architecture is the reference's FSDPViTModel (run_vit_training.py:99-162) without the wrappers: conv patch embed,
 learned position embedding, pre-LN blocks (LayerNorm eps 1e-5, optionally on q and k per head: ``cfg.qk_norm``;
 optionally LayerScale on both branches: ``cfg.init_values``), final LayerNorm (eps 1e-6), mean pool, linear head.
+With ``cfg.class_token`` it is timm's token layout instead: ``cls_token`` and ``reg_token`` in front of the patches,
+``pos_embed`` over all tokens (or the patches only, ``cfg.no_embed_class``), and the head on token 0.
 It runs on stock PyTorch ops (any device) and is meant for evaluation / export / fine-tuning outside the engine.
 """
 from __future__ import annotations
@@ -92,16 +94,30 @@ class PlainViT(nn.Module):
         super().__init__()
         self.cfg = cfg
         self.patch_embed = _PatchEmbed(cfg)
-        self.pos_embed = nn.Parameter(torch.zeros(1, cfg.num_patches, cfg.embed_dim))
+        D = cfg.embed_dim
+        self.cls_token = nn.Parameter(torch.zeros(1, 1, D)) if cfg.class_token else None
+        self.reg_token = nn.Parameter(torch.zeros(1, cfg.reg_tokens, D)) if cfg.class_token and cfg.reg_tokens else None
+        self.pos_embed = nn.Parameter(torch.zeros(1, cfg.pos_len, D))
         self.pos_drop = nn.Dropout(cfg.pos_dropout)
         self.blocks = nn.Sequential(*[_Block(cfg) for _ in range(cfg.num_blocks)])
         self.norm = nn.LayerNorm(cfg.embed_dim, eps=1e-6)
         self.head = nn.Linear(cfg.embed_dim, cfg.num_classes)
 
     def forward(self, image):
-        x = self.pos_drop(self.patch_embed(image) + self.pos_embed)
-        x = self.blocks(x)
-        return self.head(self.norm(x).mean(dim=1))
+        if self.cls_token is None:
+            x = self.pos_drop(self.patch_embed(image) + self.pos_embed)
+            x = self.blocks(x)
+            return self.head(self.norm(x).mean(dim=1))
+        x = self.patch_embed(image)
+        prefix = [self.cls_token.expand(x.shape[0], -1, -1)]
+        if self.reg_token is not None:
+            prefix.append(self.reg_token.expand(x.shape[0], -1, -1))
+        if self.cfg.no_embed_class:  # timm _pos_embed: cat(prefix, x + pos) or cat(prefix, x) + pos
+            x = torch.cat(prefix + [x + self.pos_embed], dim=1)
+        else:
+            x = torch.cat(prefix + [x], dim=1) + self.pos_embed
+        x = self.blocks(self.pos_drop(x))
+        return self.head(self.norm(x)[:, 0])
 
     @classmethod
     def from_consolidated(cls, path_or_state, cfg: ViTConfig) -> "PlainViT":

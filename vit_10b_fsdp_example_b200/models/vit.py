@@ -16,7 +16,12 @@ Architecture parity with the reference model (run_vit_training.py:99-162, timm 0
       of the un-scaled weight in one pass over the weight (ops.layer_scale_bwd)
   * optional Mixup / CutMix (timm Mixup, mode 'batch', off in the reference): drawn on the host per step (draw_mix),
     applied inside the patch im2col, with the mixed, smoothed target handled by the cross-entropy
-  * final LayerNorm(eps=1e-6), mean-pool over tokens (no CLS token), Linear head      (:151-153,159-161)
+  * optional prefix tokens (timm VisionTransformer(class_token=True, reg_tokens=R), off in the reference): a learned
+    cls_token and R reg_tokens in front of every image's N patch tokens, T = N + P tokens with P = 1 + R; pos_embed
+    covers all T tokens, or only the patches with no_embed_class.  The patch GEMM still adds the patch rows of pos_embed
+    in its epilogue; ops.tokens_fwd / tokens_bwd assemble and split the [B*T, D] token buffer
+  * final LayerNorm(eps=1e-6), mean-pool over tokens (no CLS token), Linear head      (:151-153,159-161);
+    with a class token: LayerNorm of the B class rows only (it acts per row) and the head on them
 Parameter names are timm-compatible (``norm1.weight``, ``attn.qkv.weight``, ``mlp.fc1.bias`` ...).
 
 There is no autograd here: every stage has an explicit backward, which is what lets the FSDP engine
@@ -61,11 +66,16 @@ def block_param_specs(cfg: ViTConfig) -> List[Tuple[str, Tuple[int, ...]]]:
 
 
 def root_param_specs(cfg: ViTConfig) -> List[Tuple[str, Tuple[int, ...]]]:
-    """Root unit.  The conv weight is stored as a [D, Kpad] GEMM operand (logical [D, 3, P, P])."""
+    """Root unit.  The conv weight is stored as a [D, Kpad] GEMM operand (logical [D, 3, P, P]).  The prefix tokens
+    (cls_token, reg_token) sit in front of pos_embed, as timm registers them."""
     D = cfg.embed_dim
+    prefix = [("cls_token", (1, D))] if cfg.class_token else []
+    if cfg.class_token and cfg.reg_tokens:
+        prefix.append(("reg_token", (cfg.reg_tokens, D)))
     return [
         ("patch_embed.proj.weight", (D, cfg.patch_kpad)), ("patch_embed.proj.bias", (D,)),
-        ("pos_embed", (cfg.num_patches, D)),
+        *prefix,
+        ("pos_embed", (cfg.pos_len, D)),
         ("norm.weight", (D,)), ("norm.bias", (D,)),
         ("head.weight", (cfg.num_classes, D)), ("head.bias", (cfg.num_classes,)),
     ]
@@ -73,8 +83,13 @@ def root_param_specs(cfg: ViTConfig) -> List[Tuple[str, Tuple[int, ...]]]:
 
 def logical_shapes(cfg: ViTConfig) -> Dict[str, Tuple[int, ...]]:
     """Shapes a plain timm-style (non-sharded) ViT would have for the stored tensors that differ."""
-    P = cfg.patch_size
-    return {"patch_embed.proj.weight": (cfg.embed_dim, 3, P, P), "pos_embed": (1, cfg.num_patches, cfg.embed_dim)}
+    P, D = cfg.patch_size, cfg.embed_dim
+    out = {"patch_embed.proj.weight": (D, 3, P, P), "pos_embed": (1, cfg.pos_len, D)}
+    if cfg.class_token:
+        out["cls_token"] = (1, 1, D)
+        if cfg.reg_tokens:
+            out["reg_token"] = (1, cfg.reg_tokens, D)
+    return out
 
 
 def _linear_init(out_f: int, in_f: int, gen, fan_in: Optional[int] = None, device="cpu"):
@@ -115,11 +130,16 @@ def init_root_params(cfg: ViTConfig, gen, device="cpu") -> Dict[str, torch.Tenso
     wp = torch.zeros(D, cfg.patch_kpad, device=device)
     wp[:, : cfg.patch_k] = w
     p["patch_embed.proj.weight"], p["patch_embed.proj.bias"] = wp, b
-    pos = torch.empty(cfg.num_patches, D, device=device)
+    pos = torch.empty(cfg.pos_len, D, device=device)
     torch.nn.init.trunc_normal_(pos, std=0.02, generator=gen)  # run_vit_training.py:128
     p["pos_embed"] = pos
     p["norm.weight"], p["norm.bias"] = torch.ones(D, device=device), torch.zeros(D, device=device)
     p["head.weight"], p["head.bias"] = _linear_init(cfg.num_classes, D, gen, device=device)
+    if cfg.class_token:  # timm init_weights: normal(std=1e-6), drawn after every other root draw
+        p["cls_token"] = torch.nn.init.normal_(torch.empty(1, D, device=device), std=1e-6, generator=gen)
+        if cfg.reg_tokens:
+            p["reg_token"] = torch.nn.init.normal_(torch.empty(cfg.reg_tokens, D, device=device), std=1e-6,
+                                                   generator=gen)
     return p
 
 
@@ -207,7 +227,8 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     "h" (both LayerNorm outputs), "g" (gelu(u)); True == all three.
     With cfg.qk_norm the attention runs on qkn = qk_norm(qkv).  The lean set keeps the un-normalised qkv and the norm's
     fp32 statistics; save=True also keeps qkn (a checkpoint recompute goes straight into the backward, which needs it).
-    A forward that saves nothing normalises in place."""
+    A forward that saves nothing normalises in place.
+    With prefix tokens every image has cfg.num_tokens rows (class and register tokens first); the block is unchanged."""
     do_save = save is not False and save is not None
     if save is True:
         extras = frozenset(("P", "h", "g"))
@@ -215,7 +236,7 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
         extras = frozenset()
     else:
         extras = frozenset(save)
-    N, H, hd = cfg.num_patches, cfg.num_heads, cfg.head_dim
+    N, H, hd = cfg.num_tokens, cfg.num_heads, cfg.head_dim
     pa, pm = cfg.att_dropout, cfg.mlp_dropout
     use_drop = drop is not None and drop.training and (pa > 0 or pm > 0)
     site = block_idx * 8
@@ -305,7 +326,7 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     ``ops.layer_scale_bwd`` rescales its result and yields the bias and gamma gradients, and the dgrad uses the
     folded weight.
     """
-    N, H, hd = cfg.num_patches, cfg.num_heads, cfg.head_dim
+    N, H, hd = cfg.num_tokens, cfg.num_heads, cfg.head_dim
     pa, pm = cfg.att_dropout, cfg.mlp_dropout
     masks = s["masks"]
     dpath = s.get("dpath")  # stochastic depth: per-sample scales of the (attention, MLP) branches, or None
@@ -432,14 +453,24 @@ def _qk_norm(ops, cfg: ViTConfig, p, qkv, inplace: bool):
 # Stem (patch embed + pos embed) and head (final norm, mean pool, classifier, loss)
 # ------------------------------------------------------------------------------------------------
 def stem_forward(ops, cfg: ViTConfig, p, images, dtype, drop: Optional[DropoutCtx] = None, mix: Optional[Mix] = None):
-    """mix: this step's batch mixing (``draw_mix``), applied inside the im2col; the saved cols are the mixed patches."""
+    """mix: this step's batch mixing (``draw_mix``), applied inside the im2col; the saved cols are the mixed patches.
+    With a class token the patch GEMM adds the patch rows of pos_embed and ops.tokens_fwd puts the prefix tokens in
+    front of every image: timm's cat(prefix, patches) + pos, or cat(prefix, patches + pos) with no_embed_class."""
     B = images.shape[0]
     if mix is None:
         cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype)
     else:
         cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype, mix=mix)
-    x0 = ops.linear_fwd(cols, p["patch_embed.proj.weight"], p["patch_embed.proj.bias"], residual=p["pos_embed"],
-                        res_row_mod=cfg.num_patches)
+    if cfg.class_token:
+        P, pos = cfg.num_prefix_tokens, p["pos_embed"]
+        y = ops.linear_fwd(cols, p["patch_embed.proj.weight"], p["patch_embed.proj.bias"],
+                           residual=pos if cfg.no_embed_class else pos[P:], res_row_mod=cfg.num_patches)
+        x0 = ops.tokens_fwd(y, p["cls_token"], p.get("reg_token"), None if cfg.no_embed_class else pos[:P], B,
+                            cfg.num_patches)
+        del y
+    else:
+        x0 = ops.linear_fwd(cols, p["patch_embed.proj.weight"], p["patch_embed.proj.bias"], residual=p["pos_embed"],
+                            res_row_mod=cfg.num_patches)
     mask = None  # dropout key of the position-embedding dropout (reference :129,157)
     if drop is not None and drop.training and cfg.pos_dropout > 0:
         mask = drop.key(7_000_001)
@@ -448,6 +479,9 @@ def stem_forward(ops, cfg: ViTConfig, p, images, dtype, drop: Optional[DropoutCt
 
 
 def stem_backward(ops, cfg: ViTConfig, p, G, s, dx0, dx0_colsum):
+    if cfg.class_token:
+        _stem_backward_prefix(ops, cfg, G, s, dx0)
+        return
     if s["mask"] is not None:
         dx0 = ops.dropout(dx0, cfg.pos_dropout, s["mask"])
         dx0_colsum = ops.colsum(dx0)
@@ -456,8 +490,31 @@ def stem_backward(ops, cfg: ViTConfig, p, G, s, dx0, dx0_colsum):
     G["pos_embed"].copy_(dx0.view(s["B"], cfg.num_patches, cfg.embed_dim).sum(dim=0, dtype=torch.float32))
 
 
+def _stem_backward_prefix(ops, cfg: ViTConfig, G, s, dx0):
+    """With prefix tokens: one pass (ops.tokens_bwd) splits dx0 into the patch rows, the wgrad operand, and the
+    per-token batch sums dtok [T, D], which hold the cls / reg / pos_embed gradients and, summed over the patch rows,
+    the patch bias gradient (the block-0 column sum would include the prefix rows)."""
+    if s["mask"] is not None:
+        dx0 = ops.dropout(dx0, cfg.pos_dropout, s["mask"])
+    P = cfg.num_prefix_tokens
+    dpatch, dtok = ops.tokens_bwd(dx0, s["B"], cfg.num_patches, P)
+    ops.linear_wgrad(dpatch, s["cols"], out=G["patch_embed.proj.weight"])
+    del dpatch
+    G["patch_embed.proj.bias"].copy_(dtok[P:].sum(dim=0))
+    G["pos_embed"].copy_(dtok[P:] if cfg.no_embed_class else dtok)
+    G["cls_token"].copy_(dtok[:1])
+    if cfg.reg_tokens:
+        G["reg_token"].copy_(dtok[1:P])
+
+
 def head_forward(ops, cfg: ViTConfig, p, x, B: int):
-    """logits = head(mean_tokens(norm(x)))   (run_vit_training.py:161)"""
+    """logits = head(mean_tokens(norm(x)))   (run_vit_training.py:161)
+    With a class token: logits = head(norm(x)[:, 0]); the norm acts per row, so only the B class rows are normalised."""
+    if cfg.class_token:
+        xc = x.view(B, cfg.num_tokens, cfg.embed_dim)[:, 0].contiguous()
+        xn, m, r = ops.ln_fwd(xc, p["norm.weight"], p["norm.bias"], FINAL_LN_EPS)
+        logits = ops.linear_fwd(xn, p["head.weight"], p["head.bias"])
+        return logits, dict(x=xc, m=m, r=r, pooled=xn)
     N, D = cfg.num_patches, cfg.embed_dim
     xn, m, r = ops.ln_fwd(x, p["norm.weight"], p["norm.bias"], FINAL_LN_EPS)
     pooled = ops.mean_pool(xn, B, N)
@@ -470,6 +527,13 @@ def head_backward(ops, cfg: ViTConfig, p, G, s, dlogits, B: int):
     ops.linear_wgrad(dlogits, s["pooled"], out=G["head.weight"])
     G["head.bias"].copy_(dlogits.sum(dim=0, dtype=torch.float32))
     dpooled = ops.linear_dgrad(dlogits, p["head.weight"])
+    if cfg.class_token:  # the LayerNorm backward of the B class rows, placed at token 0 of a zero [B*T, D] gradient
+        dxc, dnw, dnb, dx_sum = ops.ln_bwd(dpooled, s["x"], p["norm.weight"], s["m"], s["r"], want_dxsum=True)
+        G["norm.weight"].copy_(dnw)
+        G["norm.bias"].copy_(dnb)
+        dx = torch.zeros(B * cfg.num_tokens, D, dtype=dxc.dtype, device=dxc.device)
+        dx.view(B, cfg.num_tokens, D)[:, 0] = dxc
+        return dx, dx_sum
     dxn = ops.mean_pool_bwd(dpooled, B, N)
     dx, dnw, dnb, dx_sum = ops.ln_bwd(dxn, s["x"], p["norm.weight"], s["m"], s["r"], want_dxsum=True)
     G["norm.weight"].copy_(dnw)

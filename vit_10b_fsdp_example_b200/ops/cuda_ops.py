@@ -13,6 +13,9 @@ Every function launches hand-written kernels from ``_C.so``:
     ``qk_norm_bwd``, csrc/qk_norm.cu).
   * LayerScale: the per-channel branch scale folded into the proj / fc2 weight and bias, and its backward on the
     weight gradient (``layer_scale_fold`` / ``layer_scale_bwd``, csrc/layer_scale.cu).
+  * prefix tokens: the class / register tokens put in front of every image's patch rows, and the backward that splits
+    the token gradient into the patch rows and the per-token batch sums (``tokens_fwd`` / ``tokens_bwd``,
+    csrc/prefix_tokens.cu).
   * stochastic depth: per-sample Philox scales (``drop_path_scale``), applied as a row scale in the proj / fc2 GEMM
     epilogues, and ``drop_path_bwd`` (scaled branch gradient + its bias gradient in one pass).
 
@@ -191,6 +194,28 @@ def layer_scale_bwd(W, b, gamma, dW, S):
     out = torch.empty(2, W.shape[0], dtype=torch.float32, device=W.device)
     _C.layer_scale_bwd(W, b, gamma, dW, S, Wg, out[0], out[1])
     return Wg, out[0], out[1]
+
+
+# ------------------------------------------------------------------------------------------------
+# Prefix tokens (csrc/prefix_tokens.cu): class and register tokens in front of every image's patch rows
+# ------------------------------------------------------------------------------------------------
+def tokens_fwd(y, cls, reg, pos, B: int, N: int):
+    """x0 [B * (N + P), D] like ``torch_ops.tokens_fwd`` (reg None when there are no register tokens)."""
+    D = y.shape[1]
+    P = 1 + (reg.numel() // D if reg is not None else 0)
+    x0 = torch.empty(B * (N + P), D, dtype=y.dtype, device=y.device)
+    _C.tokens_fwd(y, cls, reg, pos, x0, B, N)
+    return x0
+
+
+def tokens_bwd(dx0, B: int, N: int, P: int):
+    """(dpatch [B * N, D] bf16, dtok [N + P, D] fp32) in one pass, like ``torch_ops.tokens_bwd``; dtok is summed over
+    the batch in a fixed order (the same bits in every run)."""
+    D = dx0.shape[1]
+    dpatch = torch.empty(B * N, D, dtype=dx0.dtype, device=dx0.device)
+    dtok = torch.empty(N + P, D, dtype=torch.float32, device=dx0.device)
+    _C.tokens_bwd(dx0, dpatch, dtok, B, N, P)
+    return dpatch, dtok
 
 
 # ------------------------------------------------------------------------------------------------

@@ -109,6 +109,32 @@ def layer_scale_bwd(W, b, gamma, dW, S):
 
 
 # ------------------------------------------------------------------------------------------------
+# Prefix tokens (timm VisionTransformer(class_token=True, reg_tokens=R)): [cls, reg_0 .. reg_{R-1}, patches] per image
+# ------------------------------------------------------------------------------------------------
+def tokens_fwd(y, cls, reg, pos, B: int, N: int):
+    """x0 [B * T, D] (T = N + P, P = 1 + R) from the patch rows y [B * N, D]: rows P .. T-1 of image b are y's rows of
+    image b, rows 0 .. P-1 are prefix[j] (+ pos[j]) summed in fp32 and rounded once, prefix = [cls [1, D], reg [R, D]]
+    (reg None when R = 0), pos [P, D] or None (prefix tokens without a position embedding)."""
+    D = y.shape[1]
+    pre = _f32(cls.reshape(1, D))
+    if reg is not None:
+        pre = torch.cat([pre, _f32(reg.reshape(-1, D))])
+    if pos is not None:
+        pre = pre + _f32(pos.reshape(-1, D))
+    P = pre.shape[0]
+    x = torch.cat([pre.to(y.dtype).expand(B, P, D), y.reshape(B, N, D)], dim=1)
+    return x.reshape(B * (N + P), D)
+
+
+def tokens_bwd(dx0, B: int, N: int, P: int):
+    """(dpatch, dtok): the patch rows of dx0 [B * T, D] as a contiguous [B * N, D] matrix, and dtok [T, D] fp32 with
+    dtok[j] = sum_b dx0[b * T + j]."""
+    D = dx0.shape[1]
+    x = dx0.reshape(B, N + P, D)
+    return x[:, P:].reshape(B * N, D).contiguous(), x.sum(dim=0, dtype=torch.float32)
+
+
+# ------------------------------------------------------------------------------------------------
 # Linear layers (timm Attention.qkv / proj, Mlp.fc1 / fc2, head) and their backward
 # ------------------------------------------------------------------------------------------------
 def gelu(x):

@@ -24,6 +24,7 @@ no cast pass.  On one GPU the gathered buffer aliases the shard itself (zero-cop
 from __future__ import annotations
 
 import contextlib
+import math
 import os
 from typing import Dict, List, Optional
 
@@ -416,12 +417,13 @@ class FSDPViT:
     def lean_bytes_per_block(self, batch: int) -> int:
         """HBM a block's lean activation set occupies: x, qkv (3), attention out, x1, fc1 pre-activation.  With QK
         normalisation the set keeps the un-normalised qkv plus the norm's fp32 mean and rstd per (token, q or k, head):
-        16 bytes per token and head (16.8 MB per ViT-10B block at 128 images, against about 3.4 GB for the rest)."""
+        16 bytes per token and head (16.8 MB per ViT-10B block at 128 images, against about 3.4 GB for the rest).
+        Every image has cfg.num_tokens rows (prefix tokens included)."""
         cfg = self.cfg
         units = 6.0 + cfg.mlp_ratio
-        n = int(batch * cfg.num_patches * cfg.embed_dim * units * torch.empty((), dtype=self.dtype).element_size())
+        n = int(batch * cfg.num_tokens * cfg.embed_dim * units * torch.empty((), dtype=self.dtype).element_size())
         if cfg.qk_norm:
-            n += 16 * batch * cfg.num_patches * cfg.num_heads
+            n += 16 * batch * cfg.num_tokens * cfg.num_heads
         return n
 
     def _auto_keep_blocks(self, batch: int) -> int:
@@ -458,12 +460,12 @@ class FSDPViT:
     def extra_bytes_per_block(self, batch: int):
         cfg = self.cfg
         es = torch.empty((), dtype=self.dtype).element_size()
-        unit = batch * cfg.num_patches * cfg.embed_dim * es
-        npad = (cfg.num_patches + 7) // 8 * 8
+        unit = batch * cfg.num_tokens * cfg.embed_dim * es
+        npad = (cfg.num_tokens + 7) // 8 * 8
         # with the fused attention pair (forward keeps the row log-sum-exp, backward rebuilds P tile by tile) there is
         # no P to keep: its budget goes to the LayerNorm outputs and gelu(u) instead
-        flash = bool(getattr(self.ops, "use_flash", lambda n, hd: False)(cfg.num_patches, cfg.head_dim))
-        p_bytes = 0 if flash else batch * cfg.num_heads * cfg.num_patches * npad * es
+        flash = bool(getattr(self.ops, "use_flash", lambda n, hd: False)(cfg.num_tokens, cfg.head_dim))
+        p_bytes = 0 if flash else batch * cfg.num_heads * cfg.num_tokens * npad * es
         return (("P", p_bytes), ("h", 2 * unit), ("g", int(cfg.mlp_ratio * unit)))
 
     def _save_mode(self, i: int, keep_from: int):
@@ -671,6 +673,7 @@ class FSDPViT:
         if has_ls and not self.cfg.init_values:
             raise ValueError("the checkpoint has ls1.gamma / ls2.gamma parameters (it was trained with LayerScale): "
                              "pass --init_values to load it (any value > 0; the learned gammas are loaded)")
+        self.check_prefix_tokens(full)
         for u in self.all_units:
             lay = u.layout
             prefix = "" if u is self.root else u.name + "."
@@ -687,6 +690,42 @@ class FSDPViT:
             self._install_master(u, shard.to(self.device))
         self.backend.params_updated()
 
+    def check_prefix_tokens(self, full: Dict[str, torch.Tensor]) -> None:
+        """Refuse a consolidated checkpoint whose prefix-token layout (class token, register tokens, rows of pos_embed)
+        does not match this model's flags, naming the flag to pass or drop.  pos_embed may hold another grid (the
+        caller resamples it); what must match is whether its first P rows belong to the prefix tokens."""
+        cfg, D = self.cfg, self.cfg.embed_dim
+        has_cls = "cls_token" in full
+        if cfg.class_token and not has_cls:
+            raise ValueError("this model uses --class_token, but the checkpoint has no cls_token: it was trained "
+                             "without a class token (drop --class_token to load it)")
+        if has_cls and not cfg.class_token:
+            raise ValueError("the checkpoint has a cls_token (it was trained with a class token): pass --class_token "
+                             "to load it")
+        n_reg = full["reg_token"].numel() // D if "reg_token" in full else 0
+        if n_reg != cfg.reg_tokens:
+            fix = f"pass --reg_tokens {n_reg}" if n_reg else "drop --reg_tokens"
+            raise ValueError(f"the checkpoint has {n_reg} register tokens (reg_token) and this model "
+                             f"{cfg.reg_tokens}: {fix} to load it")
+        if not cfg.class_token or "pos_embed" not in full:
+            return
+        rows = full["pos_embed"].numel() // D
+
+        def grid_fits(n: int) -> bool:
+            return n >= 1 and math.isqrt(n) ** 2 == n
+
+        P = cfg.num_prefix_tokens
+        if grid_fits(rows - (0 if cfg.no_embed_class else P)):
+            return
+        if cfg.no_embed_class and grid_fits(rows - P):
+            raise ValueError(f"the checkpoint's pos_embed has {rows} rows, {P} prefix tokens plus a square grid: the "
+                             f"prefix tokens were position-embedded, drop --no_embed_class to load it")
+        if cfg.class_token and not cfg.no_embed_class and grid_fits(rows):
+            raise ValueError(f"the checkpoint's pos_embed has {rows} rows, a square grid without the {P} prefix "
+                             f"tokens: pass --no_embed_class to load it")
+        want = "a square grid" if cfg.no_embed_class else f"{P} prefix rows plus a square grid"
+        raise ValueError(f"the checkpoint's pos_embed has {rows} rows, but this model needs {want}")
+
     def get_shard_metadata(self) -> dict:
         """Everything the offline consolidation tool needs to rebuild full tensors (reference utils.py:29)."""
         return {
@@ -696,7 +735,8 @@ class FSDPViT:
             "logical_shapes": {k: list(v) for k, v in vit.logical_shapes(self.cfg).items()},
             "patch_k": self.cfg.patch_k,
             "model": {k: getattr(self.cfg, k) for k in ("image_size", "patch_size", "embed_dim", "num_heads",
-                                                        "num_blocks", "mlp_ratio", "num_classes")},
+                                                        "num_blocks", "mlp_ratio", "num_classes", "class_token",
+                                                        "reg_tokens", "no_embed_class")},
         }
 
     def __repr__(self) -> str:

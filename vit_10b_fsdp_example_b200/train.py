@@ -202,11 +202,13 @@ class Trainer:
             full = torch.load(cfg.init_from_full_ckpt, map_location="cpu", weights_only=False)
             state = normalize_full_state_dict_keys(full.get("model", full))
             mcfg = self.model.cfg
+            self.model.check_prefix_tokens(state)  # before resampling: a wrong prefix layout is named, not resampled
             if "pos_embed" in state:
                 pos = state["pos_embed"]
-                state["pos_embed"] = resize_pos_embed(pos, mcfg.num_patches, mcfg.embed_dim)
+                P = 0 if mcfg.no_embed_class else mcfg.num_prefix_tokens  # rows of pos_embed that are not the grid
+                state["pos_embed"] = resize_pos_embed(pos, mcfg.num_patches, mcfg.embed_dim, num_prefix_tokens=P)
                 if state["pos_embed"] is not pos:
-                    say(f"pos_embed resampled from {pos.shape[1]} to {mcfg.num_patches} tokens (bicubic)")
+                    say(f"pos_embed resampled from {pos.shape[1] - P} to {mcfg.num_patches} tokens (bicubic)")
             self.model.load_full_state_dict(state)
             say(f"parameters initialised from the consolidated checkpoint {cfg.init_from_full_ckpt}")
             del full

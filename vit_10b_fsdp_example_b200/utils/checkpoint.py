@@ -46,23 +46,29 @@ def load_ckpt(ckpt_path: str, model, optimizer, lr_scheduler) -> None:
     print(f"resumed from checkpoint {ckpt_path}\n", end="")
 
 
-def resize_pos_embed(pos_embed: torch.Tensor, num_patches: int, embed_dim: int) -> torch.Tensor:
-    """Resample a checkpoint's ``pos_embed`` [1, g0*g0, D] to the model's [1, num_patches, D] grid, for fine-tuning at
-    another image size: bicubic, ``align_corners=False``, in fp32 over the [g0, g0, D] grid (timm's
-    ``resize_pos_embed`` for a model without a class token).  Returns ``pos_embed`` itself when the grids match."""
+def resize_pos_embed(pos_embed: torch.Tensor, num_patches: int, embed_dim: int,
+                     num_prefix_tokens: int = 0) -> torch.Tensor:
+    """Resample a checkpoint's ``pos_embed`` [1, P + g0*g0, D] to the model's [1, P + num_patches, D], for fine-tuning
+    at another image size: the first P = ``num_prefix_tokens`` rows (class / register tokens) pass through unchanged and
+    the grid rows are resampled bicubically, ``align_corners=False``, in fp32 over the [g0, g0, D] grid (timm's
+    ``resize_pos_embed`` with ``num_tokens``; later timm releases call it ``resample_abs_pos_embed`` and antialias by
+    default, which this does not).  Returns ``pos_embed`` itself when the grids match."""
     if pos_embed.dim() != 3 or pos_embed.shape[0] != 1:
         raise ValueError(f"pos_embed: expected shape [1, N, D], got {tuple(pos_embed.shape)}")
-    n0, d0 = pos_embed.shape[1], pos_embed.shape[2]
+    P = num_prefix_tokens
+    n0, d0 = pos_embed.shape[1] - P, pos_embed.shape[2]
     if d0 != embed_dim:
         raise ValueError(f"pos_embed: checkpoint embed dim {d0} does not match the model's {embed_dim}")
     if n0 == num_patches:
         return pos_embed
-    g0, g = math.isqrt(n0), math.isqrt(num_patches)
-    if g0 * g0 != n0 or g * g != num_patches:
-        raise ValueError(f"pos_embed: cannot resample {n0} to {num_patches} tokens: both must be square grids")
-    grid = pos_embed.detach().float().reshape(1, g0, g0, d0).permute(0, 3, 1, 2)
+    g0, g = math.isqrt(max(n0, 0)), math.isqrt(num_patches)
+    if n0 < 1 or g0 * g0 != n0 or g * g != num_patches:
+        after = f" after its {P} prefix rows" if P else ""
+        raise ValueError(f"pos_embed: cannot resample {n0} to {num_patches} tokens{after}: both must be square grids")
+    grid = pos_embed[:, P:].detach().float().reshape(1, g0, g0, d0).permute(0, 3, 1, 2)
     grid = torch.nn.functional.interpolate(grid, size=(g, g), mode="bicubic", align_corners=False)
-    return grid.permute(0, 2, 3, 1).reshape(1, num_patches, d0).to(pos_embed.dtype)
+    grid = grid.permute(0, 2, 3, 1).reshape(1, num_patches, d0).to(pos_embed.dtype)
+    return torch.cat([pos_embed[:, :P].detach(), grid], dim=1) if P else grid
 
 
 _WRAPPER_PARTS =("_fsdp_wrapped_module.", "_fpw_module.", "_checkpoint_wrapped_module.", "_orig_mod.")
