@@ -101,7 +101,21 @@ def build_arg_parser() -> argparse.ArgumentParser:
     parser.add_argument("--no_embed_class", action="store_true",
                         help="pos_embed covers the patches only and the class / register tokens get no position "
                              "embedding (timm no_embed_class=True); needs --class_token")
+    parser.add_argument("--swiglu", action="store_true",
+                        help="SwiGLU MLP (timm mlp_layer=SwiGLUPacked, act_layer=nn.SiLU; Shazeer 2020, DINOv2-g): "
+                             "fc1 makes Hd = int(embed_dim * mlp_ratio) features [gate | value], fc2 reads "
+                             "silu(gate) * value of width Hd / 2; Hd must be a multiple of 16")
     return parser
+
+
+def check_swiglu(cfg) -> None:
+    """The SwiGLU value half starts at column Hd / 2 of the packed fc1 output: the GEMM's second store map and the
+    16-byte vectors of the SwiGLU kernels need that column 16-byte aligned, so Hd % 16 == 0 (timm only needs Hd even)."""
+    if getattr(cfg, "swiglu", False):
+        hd = int(cfg.embed_dim * cfg.mlp_ratio)
+        if hd % 16 != 0:
+            raise ValueError(f"--swiglu needs the MLP width Hd = int(embed_dim * mlp_ratio) to be a multiple of 16 "
+                             f"(the value half starts at column Hd / 2, which must be 16-byte aligned); got Hd = {hd}")
 
 
 def check_prefix_flags(args) -> None:
@@ -156,6 +170,7 @@ def parse_args(argv=None) -> argparse.Namespace:
     args = parser.parse_args(argv)
     try:
         check_prefix_flags(args)
+        check_swiglu(args)
     except ValueError as e:
         parser.error(str(e))
     return args
@@ -184,6 +199,7 @@ class ViTConfig:
     class_token: bool = False  # learned cls_token in front of the patches, classified from (timm global_pool='token')
     reg_tokens: int = 0  # learned register tokens after the class token (needs class_token)
     no_embed_class: bool = False  # pos_embed covers the patches only (timm no_embed_class=True; needs class_token)
+    swiglu: bool = False  # SwiGLU MLP (timm SwiGLUPacked): fc1 -> [gate | value] of width hidden_dim, fc2 reads half of it
 
     def __post_init__(self):
         if not 0.0 <= self.drop_path_rate < 1.0:
@@ -202,6 +218,7 @@ class ViTConfig:
         if not (isinstance(self.reg_tokens, int) and self.reg_tokens >= 0):
             raise ValueError(f"reg_tokens must be an integer >= 0, got {self.reg_tokens}")
         check_prefix_flags(self)
+        check_swiglu(self)
 
     @property
     def mixing(self) -> bool:
@@ -218,7 +235,8 @@ class ViTConfig:
                    mixup_prob=getattr(cfg, "mixup_prob", 1.0), mixup_switch_prob=getattr(cfg, "mixup_switch_prob", 0.5),
                    smoothing=getattr(cfg, "smoothing", 0.0), qk_norm=getattr(cfg, "qk_norm", False),
                    init_values=getattr(cfg, "init_values", 0.0), class_token=getattr(cfg, "class_token", False),
-                   reg_tokens=getattr(cfg, "reg_tokens", 0), no_embed_class=getattr(cfg, "no_embed_class", False))
+                   reg_tokens=getattr(cfg, "reg_tokens", 0), no_embed_class=getattr(cfg, "no_embed_class", False),
+                   swiglu=getattr(cfg, "swiglu", False))
 
     @property
     def grid(self) -> int:
@@ -254,6 +272,11 @@ class ViTConfig:
         return int(self.embed_dim * self.mlp_ratio)
 
     @property
+    def mlp_out_dim(self) -> int:
+        """Width of the fc2 input: hidden_dim, or with SwiGLU the hidden_dim / 2 columns of silu(gate) * value."""
+        return self.hidden_dim // 2 if self.swiglu else self.hidden_dim
+
+    @property
     def patch_k(self) -> int:
         return 3 * self.patch_size * self.patch_size
 
@@ -266,7 +289,7 @@ class ViTConfig:
         D, Hd = self.embed_dim, self.hidden_dim
         qk = 4 * self.head_dim if self.qk_norm else 0  # q_norm / k_norm weight and bias
         ls = 2 * D if self.init_values else 0  # ls1.gamma / ls2.gamma
-        return 2 * D + (3 * D * D + 3 * D) + qk + (D * D + D) + 2 * D + (Hd * D + Hd) + (D * Hd + D) + ls
+        return 2 * D + (3 * D * D + 3 * D) + qk + (D * D + D) + 2 * D + (Hd * D + Hd) + (D * self.mlp_out_dim + D) + ls
 
     def root_numel(self) -> int:
         D = self.embed_dim
@@ -279,6 +302,6 @@ class ViTConfig:
     def flops_per_image(self, grad_ckpt: bool = True) -> float:
         """Matmul FLOPs of one training step per image (fwd + bwd [+ recompute])."""
         D, Hd, N, T = self.embed_dim, self.hidden_dim, self.num_patches, self.num_tokens
-        per_block = 2 * T * (3 * D * D + D * D + 2 * D * Hd) + 4 * T * T * D
+        per_block = 2 * T * (3 * D * D + D * D + D * Hd + D * self.mlp_out_dim) + 4 * T * T * D
         fwd = self.num_blocks * per_block + 2 * N * self.patch_k * D + 2 * D * self.num_classes
         return fwd * (4.0 if grad_ckpt else 3.0)

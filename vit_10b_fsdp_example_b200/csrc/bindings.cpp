@@ -205,6 +205,22 @@ void dgelu_mul(Tensor dg, Tensor u, Tensor du) {
     c10::cuda::CUDAGuard guard(u.device());
     b200::dgelu_mul(bf16_ptr(dg), bf16_ptr(u), bf16_mut(du), u.numel(), cur_stream());
 }
+// u [M, Hd] packed [gate | value]; g [M, Hd / 2]; dg [M, Hd / 2]; du [M, Hd]; all contiguous.
+void swiglu_fwd(Tensor u, Tensor g) {
+    c10::cuda::CUDAGuard guard(u.device());
+    TORCH_CHECK(u.dim() == 2 && g.dim() == 2 && u.is_contiguous() && g.is_contiguous(),
+                "swiglu_fwd: contiguous 2-D u and g");
+    TORCH_CHECK(g.size(0) == u.size(0) && 2 * g.size(1) == u.size(1), "swiglu_fwd: g must be [M, Hd / 2] for u [M, Hd]");
+    b200::swiglu_fwd(bf16_ptr(u), bf16_mut(g), u.size(0), u.size(1), cur_stream());
+}
+void swiglu_bwd(Tensor dg, Tensor u, Tensor du) {
+    c10::cuda::CUDAGuard guard(u.device());
+    TORCH_CHECK(u.dim() == 2 && dg.dim() == 2 && du.dim() == 2 && u.is_contiguous() && dg.is_contiguous() &&
+                    du.is_contiguous(), "swiglu_bwd: contiguous 2-D dg, u and du");
+    TORCH_CHECK(dg.size(0) == u.size(0) && 2 * dg.size(1) == u.size(1) && du.sizes() == u.sizes(),
+                "swiglu_bwd: dg must be [M, Hd / 2] and du [M, Hd] for u [M, Hd]");
+    b200::swiglu_bwd(bf16_ptr(dg), bf16_ptr(u), bf16_mut(du), u.size(0), u.size(1), cur_stream());
+}
 
 // qkv / out: [T, >= 3 H hd] row-major bf16 (out may be qkv: in place); mean / rstd: fp32 [T * 2 * H].
 void qk_norm_fwd(Tensor qkv, Tensor wq, Tensor bq, Tensor wk, Tensor bk, Tensor out, Tensor mean, Tensor rstd,
@@ -476,6 +492,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
           py::arg("box") = std::vector<int64_t>());
     m.def("gelu_fwd", &gelu_fwd);
     m.def("dgelu_mul", &dgelu_mul);
+    m.def("swiglu_fwd", &swiglu_fwd);
+    m.def("swiglu_bwd", &swiglu_bwd);
     m.def("dropout", &dropout);
     m.def("drop_path_scale", &drop_path_scale);
     m.def("drop_path_bwd", &drop_path_bwd);

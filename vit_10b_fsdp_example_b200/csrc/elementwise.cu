@@ -475,6 +475,59 @@ __global__ void __launch_bounds__(256) dgelu_mul_kernel(const __nv_bfloat16* __r
 }
 
 // ------------------------------------------------------------------------------------------------
+// Stand-alone SwiGLU (timm SwiGLUPacked): u = [gate | value] [M, 2H'], g = silu(gate) * value [M, H'].  The short-K
+// counterparts of the GEMM's SwiGLU / dSwiGLU epilogues, and the re-materialisation of g in backward.  One thread owns 8
+// adjacent columns of one row (16-byte vectors of the gate, the value and the output); sigmoid is rcp.approx(1 + exp(-x)),
+// exactly as in the GEMM epilogue, so the fused and unfused routes compute the same function.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float swiglu_sigmoid(float x) {
+    float r;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + __expf(-x)));
+    return r;
+}
+
+__global__ void __launch_bounds__(256) swiglu_fwd_kernel(const __nv_bfloat16* __restrict__ u,
+                                                         __nv_bfloat16* __restrict__ g, int64_t M, int hvec) {
+    // rows over grid.y, 16-byte column vectors over grid.x: no 64-bit division (it would be a subroutine call)
+    for (int64_t row = blockIdx.y; row < M; row += gridDim.y)
+        for (int cv = blockIdx.x * blockDim.x + threadIdx.x; cv < hvec; cv += gridDim.x * blockDim.x) {
+        const int64_t i = row * hvec + cv;
+        const uint4* ur = reinterpret_cast<const uint4*>(u) + row * 2 * hvec;
+        float a[8], b[8];
+        unpack8(ur[cv], a);
+        unpack8(ur[hvec + cv], b);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) b[q] *= a[q] * swiglu_sigmoid(a[q]);
+        reinterpret_cast<uint4*>(g)[i] = pack8(b);
+    }
+}
+
+__global__ void __launch_bounds__(256) swiglu_bwd_kernel(const __nv_bfloat16* __restrict__ dg,
+                                                         const __nv_bfloat16* __restrict__ u,
+                                                         __nv_bfloat16* __restrict__ du, int64_t M, int hvec) {
+    // rows over grid.y, 16-byte column vectors over grid.x: no 64-bit division (it would be a subroutine call)
+    for (int64_t row = blockIdx.y; row < M; row += gridDim.y)
+        for (int cv = blockIdx.x * blockDim.x + threadIdx.x; cv < hvec; cv += gridDim.x * blockDim.x) {
+        const int64_t i = row * hvec + cv;
+        const uint4* ur = reinterpret_cast<const uint4*>(u) + row * 2 * hvec;
+        float a[8], b[8], d[8];
+        unpack8(ur[cv], a);
+        unpack8(ur[hvec + cv], b);
+        unpack8(reinterpret_cast<const uint4*>(dg)[i], d);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+            const float s = swiglu_sigmoid(a[q]);
+            const float dq = d[q];
+            d[q] = dq * b[q] * (s * fmaf(a[q], 1.0f - s, 1.0f));  // du_gate = dg * b * silu'(a)
+            b[q] = dq * (a[q] * s);                               // du_val  = dg * silu(a)
+        }
+        uint4* dr = reinterpret_cast<uint4*>(du) + row * 2 * hvec;
+        dr[cv] = pack8(d);
+        dr[hvec + cv] = pack8(b);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Dropout on the kernel path (reference flags --pos_dropout / --att_dropout / --mlp_dropout, run_vit_training.py:
 // 345-347): y = x * keep / (1 - p) with keep drawn from Philox-4x32-10, counter = index of the 16-byte vector, key =
 // the 64-bit (seed, step, site) key of the engine's DropoutCtx.  The mask is a pure function of (key, element index),
@@ -1352,6 +1405,35 @@ void dgelu_mul(const __nv_bfloat16* dg, const __nv_bfloat16* u, __nv_bfloat16* d
     if (grid == 0) return;
     dgelu_mul_kernel<<<grid, 256, 0, stream>>>(dg, u, du, n / 8);
     check_launch("dgelu_mul");
+}
+
+void swiglu_fwd(const __nv_bfloat16* u, __nv_bfloat16* g, int64_t M, int64_t hidden, cudaStream_t stream) {
+    if (M < 0 || hidden < 0 || hidden % 16 != 0)
+        throw std::runtime_error("swiglu_fwd: the packed width Hd must be a multiple of 16 (16-byte halves)");
+    if ((reinterpret_cast<uintptr_t>(u) | reinterpret_cast<uintptr_t>(g)) & 15)
+        throw std::runtime_error("swiglu_fwd: u and g must be 16-byte aligned");
+    const int hvec = static_cast<int>(hidden / 16);
+    if (M == 0 || hvec == 0) return;
+    const int gx = std::min((hvec + 255) / 256, 64);
+    const int64_t gy = std::min<int64_t>(std::min<int64_t>(M, std::max(1, sm_count() * 16 / gx)), 65535);
+    const dim3 grid(gx, static_cast<unsigned>(gy));
+    swiglu_fwd_kernel<<<grid, 256, 0, stream>>>(u, g, M, hvec);
+    check_launch("swiglu_fwd");
+}
+
+void swiglu_bwd(const __nv_bfloat16* dg, const __nv_bfloat16* u, __nv_bfloat16* du, int64_t M, int64_t hidden,
+                cudaStream_t stream) {
+    if (M < 0 || hidden < 0 || hidden % 16 != 0)
+        throw std::runtime_error("swiglu_bwd: the packed width Hd must be a multiple of 16 (16-byte halves)");
+    if ((reinterpret_cast<uintptr_t>(dg) | reinterpret_cast<uintptr_t>(u) | reinterpret_cast<uintptr_t>(du)) & 15)
+        throw std::runtime_error("swiglu_bwd: dg, u and du must be 16-byte aligned");
+    const int hvec = static_cast<int>(hidden / 16);
+    if (M == 0 || hvec == 0) return;
+    const int gx = std::min((hvec + 255) / 256, 64);
+    const int64_t gy = std::min<int64_t>(std::min<int64_t>(M, std::max(1, sm_count() * 16 / gx)), 65535);
+    const dim3 grid(gx, static_cast<unsigned>(gy));
+    swiglu_bwd_kernel<<<grid, 256, 0, stream>>>(dg, u, du, M, hvec);
+    check_launch("swiglu_bwd");
 }
 
 void dropout(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, float p, uint64_t key, cudaStream_t stream) {

@@ -41,6 +41,11 @@ void layernorm_bwd_stream(const __nv_bfloat16* dy, const __nv_bfloat16* x, const
                           float* dxsum, int rows, int D, cudaStream_t stream);
 void gelu_fwd(const __nv_bfloat16* u, __nv_bfloat16* g, int64_t n, cudaStream_t stream);
 void dgelu_mul(const __nv_bfloat16* dg, const __nv_bfloat16* u, __nv_bfloat16* du, int64_t n, cudaStream_t stream);
+// SwiGLU on a packed u = [gate | value] [M, hidden] (row-major, hidden % 16 == 0, 16-byte aligned):
+// g [M, hidden / 2] = silu(gate) * value;  du [M, hidden] = [dg * value * silu'(gate) | dg * silu(gate)].
+void swiglu_fwd(const __nv_bfloat16* u, __nv_bfloat16* g, int64_t M, int64_t hidden, cudaStream_t stream);
+void swiglu_bwd(const __nv_bfloat16* dg, const __nv_bfloat16* u, __nv_bfloat16* du, int64_t M, int64_t hidden,
+                cudaStream_t stream);
 // y = x * keep / (1 - p), keep = Philox-4x32-10(key, vector index): a pure function of (key, position), so recompute and
 // backward regenerate the mask.  p is quantised to 1/65536.  y may alias x.
 void dropout(const __nv_bfloat16* x, __nv_bfloat16* y, int64_t n, float p, uint64_t key, cudaStream_t stream);

@@ -1,8 +1,8 @@
 // Persistent, warp-specialised bf16 GEMM for sm_90a (H100):
 //   TMA (cp.async.bulk.tensor, SWIZZLE_128B)  ->  shared-memory ring (mbarrier full / empty pairs)
 //   wgmma.mma_async m64 x BLOCK_N x 16, two consumer warpgroups per CTA, fp32 accumulators in registers
-//   fused epilogue (bias, exact GELU, dGELU, per-row scale, residual add, pre-activation side output,
-//   bias-gradient column sums)  ->  swizzled smem  ->  TMA store.
+//   fused epilogue (bias, exact GELU, dGELU, SwiGLU, dSwiGLU, per-row scale, residual add, pre-activation side
+//   output, bias-gradient column sums)  ->  swizzled smem  ->  TMA store.
 //
 // One CTA owns a 128 x BLOCK_N output tile; a producer warp (with a reduced register budget) keeps the ring
 // full while the consumer warpgroups (each 64 rows of the tile) issue the MMAs and run the epilogue.
@@ -108,6 +108,9 @@ __device__ __forceinline__ float dgelu_erf(float x) {
     const float cdf = 0.5f * (1.0f + erf_as(x * 0.70710678118654752f, e));
     return fmaf(x * 0.3989422804014327f, e, cdf);  // cdf + x * pdf,  pdf = exp(-x^2/2)/sqrt(2 pi)
 }
+// sigmoid(x) = 1 / (1 + exp(-x)) with ex2.approx and rcp.approx: no call.  exp(-x) overflows to inf for x < -88 and the
+// reciprocal of inf is 0, so silu(x) = x * sigmoid(x) and silu'(x) = s (1 + x (1 - s)) go to -0 / 0 there, as they should.
+__device__ __forceinline__ float sigmoid_approx(float x) { return rcp_approx(1.0f + __expf(-x)); }
 
 // kClusterM = 2: CTAs run in (2, 1, 1) clusters.  The two CTAs of a cluster own m-tiles 2 mp and 2 mp + 1 of the same
 // (batch, n-tile), so they need the same B tile: each producer loads its own A tile and one half of B, multicast to
@@ -120,17 +123,26 @@ __device__ __forceinline__ float dgelu_erf(float x) {
 //                producer's multicast writes stage s of the peer as well and may start only once both released it.
 // Both CTAs walk the same tile sequence, so they fill and drain the ring in lock step; cluster syncs after barrier
 // init and before exit keep a CTA from multicasting into, or arriving on, a peer that has not started or has left.
-template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM, bool kRowScale>
-__global__ void __launch_bounds__(kNumThreads, 1)
-    gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                          const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_aux,
-                          const KernelParams p) {
+//
+// kGlu (kActSwiglu / kActDSwiglu, 0 otherwise) selects a SwiGLU epilogue (gemm_sm90.h).  A template flag like kRowScale:
+// the instantiations with kGlu = 0 compile exactly as they did before the SwiGLU epilogues existed.  The forward GLU
+// tile is BLOCK_N / 2 output columns wide: its B stage holds the gate rows [n, n + BLOCK_N / 2) in the lower half and
+// the value rows [N + n, ...) in the upper half (with kClusterM = 2, CTA rank 0 loads the gate half and rank 1 the value
+// half, at the stage offsets of the plain multicast), so accumulator column j and j + BLOCK_N / 2 pair up in registers.
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM, bool kRowScale, int kGlu>
+__device__ __forceinline__ void gemm_bf16_sm90_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b,
+                                                    const CUtensorMap& tmap_d, const CUtensorMap& tmap_aux,
+                                                    const KernelParams& p) {
     constexpr int kABytes = kBlockM * kBlockK * 2;
     constexpr int kBBytes = BLOCK_N * kBlockK * 2;
     constexpr int kStageBytes = kABytes + kBBytes;
+    constexpr int kTileN = kGlu == kActSwiglu ? BLOCK_N / 2 : BLOCK_N;  // output columns per tile
     static_assert(BLOCK_N % 64 == 0 && BLOCK_N <= 256, "epilogue works in 64-column chunks; wgmma N <= 256");
     static_assert(kABytes % 1024 == 0 && kBBytes % 1024 == 0, "swizzle-128B needs 1024 B aligned stages");
     static_assert(kClusterM == 1 || (kClusterM == 2 && BLOCK_N % 128 == 0), "B splits into two 64-row multiples");
+    static_assert(kGlu != kActSwiglu || (kMajorA == 0 && kMajorB == 0 && BLOCK_N % 128 == 0 && !kRowScale),
+                  "SwiGLU forward: K-major operands, gate / value halves of 64-row multiples");
+    static_assert(kGlu != kActDSwiglu || (kMajorA == 0 && kMajorB == 1 && !kRowScale), "dSwiGLU: the fc2 dgrad (NN)");
 
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t* smem_cd = smem;
@@ -204,7 +216,7 @@ __global__ void __launch_bounds__(kNumThreads, 1)
                     decode_tile(t, b, mt, nt);
                     const int bi = b % p.nb_inner, bo = b / p.nb_inner;
                     const int m_idx = mt * kBlockM;
-                    const int n_idx = nt * BLOCK_N;
+                    const int n_idx = nt * kTileN;
                     if (p.ag.world > 1) {
                         // B rows [n_idx, n_idx + BLOCK_N) must have been pulled into the local gathered buffer
                         const int last_row = min(n_idx + BLOCK_N, p.N) - 1;
@@ -234,7 +246,21 @@ __global__ void __launch_bounds__(kNumThreads, 1)
                                 tma_load_4d(&tmap_a, &full_bar[stage], sa + i * (64 * kBlockK * 2), m_idx + i * 64,
                                                  k_idx, bi, bo);
                         }
-                        if constexpr (kClusterM == 1) {
+                        if constexpr (kGlu == kActSwiglu) {
+                            // gate rows [n_idx, +BLOCK_N / 2) -> lower half, value rows [N + n_idx, ...) -> upper half.
+                            // Gate rows past N are value rows (their columns are discarded), value rows past 2N are
+                            // zero-filled by TMA, so any N works.
+                            constexpr int kHalfN = BLOCK_N / 2;
+                            if constexpr (kClusterM == 1) {
+                                tma_load_4d(&tmap_b, &full_bar[stage], sb, k_idx, n_idx, bi, bo);
+                                tma_load_4d(&tmap_b, &full_bar[stage], sb + kHalfN * (kBlockK * 2), k_idx, p.N + n_idx,
+                                            bi, bo);
+                            } else {
+                                const int r = cta_rank();
+                                tma_load_4d_multicast(&tmap_b, &full_bar[stage], sb + r * kHalfN * (kBlockK * 2), k_idx,
+                                                      n_idx + r * p.N, bi, bo, 0b11);
+                            }
+                        } else if constexpr (kClusterM == 1) {
                             if constexpr (kMajorB == 0) {
                                 tma_load_4d(&tmap_b, &full_bar[stage], sb, k_idx, n_idx, bi, bo);
                             } else {
@@ -335,7 +361,7 @@ __global__ void __launch_bounds__(kNumThreads, 1)
             decode_tile(t, b, mt, nt);
             const int bi = b % p.nb_inner, bo = b / p.nb_inner;
             const int m0 = mt * kBlockM + cw * 64;
-            const int n0 = nt * BLOCK_N;
+            const int n0 = nt * kTileN;
 
             uint32_t prev_stage = 0;
             for (int kb = 0; kb < num_kb; ++kb) {
@@ -364,104 +390,251 @@ __global__ void __launch_bounds__(kNumThreads, 1)
             // ---- epilogue: registers -> swizzled staging buffer -> TMA store, 64 columns at a time ----
             const int row0 = m0 + static_cast<int>(wrow), row1 = row0 + 8;
             const bool row0_ok = row0 < p.M, row1_ok = row1 < p.M;
-            const __nv_bfloat16 *ext0 = nullptr, *ext1 = nullptr;
-            if (ext_is_aux) {
-                ext0 = e.aux_in + static_cast<int64_t>(row0) * e.ld_aux;
-                ext1 = e.aux_in + static_cast<int64_t>(row1) * e.ld_aux;
-            } else if (e.residual != nullptr) {
-                ext0 = e.residual + static_cast<int64_t>(e.res_row_mod > 0 ? row0 % e.res_row_mod : row0) * e.ld_res;
-                ext1 = e.residual + static_cast<int64_t>(e.res_row_mod > 0 ? row1 % e.res_row_mod : row1) * e.ld_res;
-            }
-            // kRowScale (stochastic depth): v = (acc + bias) * row_scale[row / rows_per_scale] before the residual add,
-            // the scale read once per accumulator row of the tile.  A template flag rather than a run-time branch: the
-            // GELU / dGELU epilogues run at the register limit, and any change to their code changes how ptxas
-            // schedules them; the instantiations without the flag compile exactly as they would without the feature.
-            float rs0 = 1.f, rs1 = 1.f;
-            if constexpr (kRowScale) {
-                if (row0_ok) rs0 = __ldg(e.row_scale + row0 / e.rows_per_scale);
-                if (row1_ok) rs1 = __ldg(e.row_scale + row1 / e.rows_per_scale);
-            }
+            if constexpr (kGlu == kActSwiglu) {
+                // gate of output column n in accumulator chunk c, its value in chunk c + kHalfChunks
+                constexpr int kHalfChunks = BLOCK_N / 128;
+                auto gate_value = [&](int c, int j, float (&a)[4], float (&v)[4]) {
 #pragma unroll
-            for (int c = 0; c < BLOCK_N / 64; ++c) {
-                const int ncol0 = n0 + c * 64;
-                if (ncol0 >= p.N) continue;  // warpgroup-uniform: nothing to store
-                uint8_t* buf0 = grp_buf + (e.has_aux_out ? 0 : (flip & 1)) * kCdBufBytes;
-                uint8_t* buf1 = grp_buf + kCdBufBytes;
-                if (etid == 0) {  // staging buffer(s) of this warpgroup free again?
-                    if (e.has_aux_out)
-                        tma_store_wait_read<0>();
-                    else
+                    for (int q = 0; q < 4; ++q) a[q] = d[(c * 8 + j) * 4 + q], v[q] = d[((c + kHalfChunks) * 8 + j) * 4 + q];
+                };
+#pragma unroll
+                for (int c = 0; c < kHalfChunks; ++c) {
+                    const int ncol0 = n0 + c * 64;
+                    if (ncol0 >= p.N) continue;  // warpgroup-uniform
+                    // both biases go into the accumulators in place: no bias value stays live across the two passes
+                    if (e.bias != nullptr) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const int col = ncol0 + j * 8 + static_cast<int>(cpair);
+                            if (col < p.N) {
+                                const uint32_t bg = __ldg(reinterpret_cast<const uint32_t*>(e.bias + col));
+                                const uint32_t bv = __ldg(reinterpret_cast<const uint32_t*>(e.bias + p.N + col));
+                                float* dg = d + (c * 8 + j) * 4;
+                                float* dv = d + ((c + kHalfChunks) * 8 + j) * 4;
+                                dg[0] += bf16_lo(bg), dg[1] += bf16_hi(bg), dg[2] += bf16_lo(bg), dg[3] += bf16_hi(bg);
+                                dv[0] += bf16_lo(bv), dv[1] += bf16_hi(bv), dv[2] += bf16_lo(bv), dv[3] += bf16_hi(bv);
+                            }
+                        }
+                    }
+                    // Three outputs per chunk and two staging buffers: the pre-activations go first (gate -> buffer 0,
+                    // value -> buffer 1, stored to the two [M, N] halves of u through the aux map's batch index), then
+                    // g reuses buffer 0 once the TMA engine has read it.  Without them g alternates between buffers.
+                    if (e.has_aux_out) {
+                        if (etid == 0) tma_store_wait_read<0>();
+                        named_bar_sync(bar_id, kEpiThreads);
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            float a[4], v[4];
+                            gate_value(c, j, a, v);
+                            const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
+                            st_shared_b32(smem_u32(grp_buf) + off0, pack_bf16x2(a[0], a[1]));
+                            st_shared_b32(smem_u32(grp_buf) + off0 + 8 * 128, pack_bf16x2(a[2], a[3]));
+                            st_shared_b32(smem_u32(grp_buf + kCdBufBytes) + off0, pack_bf16x2(v[0], v[1]));
+                            st_shared_b32(smem_u32(grp_buf + kCdBufBytes) + off0 + 8 * 128, pack_bf16x2(v[2], v[3]));
+                        }
+                        fence_proxy_async_smem();
+                        named_bar_sync(bar_id, kEpiThreads);
+                        if (etid == 0) {
+                            tma_store_4d(&tmap_aux, grp_buf, ncol0, m0, 0, 0);
+                            tma_store_4d(&tmap_aux, grp_buf + kCdBufBytes, ncol0, m0, 1, 0);
+                            tma_store_commit();
+                            tma_store_wait_read<0>();
+                        }
+                    } else if (etid == 0) {
                         tma_store_wait_read<1>();
-                }
-                named_bar_sync(bar_id, kEpiThreads);
+                    }
+                    named_bar_sync(bar_id, kEpiThreads);
+                    uint8_t* buf0 = grp_buf + (e.has_aux_out ? 0 : (flip & 1)) * kCdBufBytes;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int col = ncol0 + j * 8 + static_cast<int>(cpair);
-                    const bool c0_ok = col < p.N, c1_ok = col + 1 < p.N;
-                    float v[4] = {d[(c * 8 + j) * 4], d[(c * 8 + j) * 4 + 1], d[(c * 8 + j) * 4 + 2], d[(c * 8 + j) * 4 + 3]};
-                    uint32_t x0 = 0, x1 = 0;  // dGELU pre-activation or residual of (row0 | row1, col..col+1)
-                    if (ext0 != nullptr && c0_ok) {
-                        if (row0_ok) x0 = __ldg(reinterpret_cast<const uint32_t*>(ext0 + col));
-                        if (row1_ok) x1 = __ldg(reinterpret_cast<const uint32_t*>(ext1 + col));
-                    }
-                    if (e.bias != nullptr && c0_ok) {
-                        const uint32_t bw = __ldg(reinterpret_cast<const uint32_t*>(e.bias + col));
-                        v[0] += bf16_lo(bw), v[1] += bf16_hi(bw), v[2] += bf16_lo(bw), v[3] += bf16_hi(bw);
-                    }
-                    // 16-byte chunk j of a 128-byte row, XOR-swizzled with the row like the TMA store expects
-                    const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
-                    const uint32_t off1 = off0 + 8 * 128;  // row + 8 has the same (row & 7)
-                    if (e.has_aux_out) {
-                        st_shared_b32(smem_u32(buf1) + off0, pack_bf16x2(v[0], v[1]));
-                        st_shared_b32(smem_u32(buf1) + off1, pack_bf16x2(v[2], v[3]));
-                    }
-                    if (e.act == kActGelu) {
+                    for (int j = 0; j < 8; ++j) {
+                        float a[4], v[4];
+                        gate_value(c, j, a, v);
 #pragma unroll
-                        for (int q = 0; q < 4; ++q) v[q] = gelu_erf(v[q]);
-                    } else if (ext_is_aux) {
-                        v[0] *= dgelu_erf(bf16_lo(x0)), v[1] *= dgelu_erf(bf16_hi(x0));
-                        v[2] *= dgelu_erf(bf16_lo(x1)), v[3] *= dgelu_erf(bf16_hi(x1));
+                        for (int q = 0; q < 4; ++q) v[q] *= a[q] * sigmoid_approx(a[q]);
+                        const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
+                        st_shared_b32(smem_u32(buf0) + off0, pack_bf16x2(v[0], v[1]));
+                        st_shared_b32(smem_u32(buf0) + off0 + 8 * 128, pack_bf16x2(v[2], v[3]));
                     }
-                    if constexpr (kRowScale) {  // host: only with kActNone, so this is (acc + bias) * scale
-                        v[0] *= rs0, v[1] *= rs0, v[2] *= rs1, v[3] *= rs1;
+                    fence_proxy_async_smem();
+                    named_bar_sync(bar_id, kEpiThreads);
+                    if (etid == 0) {
+                        tma_store_4d(&tmap_d, buf0, ncol0, m0, bi, bo);
+                        tma_store_commit();
                     }
-                    if (e.residual != nullptr && !ext_is_aux) {
-                        v[0] += bf16_lo(x0), v[1] += bf16_hi(x0), v[2] += bf16_lo(x1), v[3] += bf16_hi(x1);
-                    }
-                    // rows / columns outside the problem are clipped by the TMA store; zeros keep the column sums clean
-                    if (!(row0_ok && c0_ok)) v[0] = 0.f;
-                    if (!(row0_ok && c1_ok)) v[1] = 0.f;
-                    if (!(row1_ok && c0_ok)) v[2] = 0.f;
-                    if (!(row1_ok && c1_ok)) v[3] = 0.f;
-                    st_shared_b32(smem_u32(buf0) + off0, pack_bf16x2(v[0], v[1]));
-                    st_shared_b32(smem_u32(buf0) + off1, pack_bf16x2(v[2], v[3]));
+                    ++flip;
                 }
-                fence_proxy_async_smem();
-                named_bar_sync(bar_id, kEpiThreads);
-                if (etid == 0) {
-                    tma_store_4d(&tmap_d, buf0, ncol0, m0, bi, bo);
-                    tma_store_commit();
-                    if (e.has_aux_out) {
+            } else if constexpr (kGlu == kActDSwiglu) {
+                // acc = dh[m, n]; a = u[m, n] (gate), b = u[m, N + n] (value).  du_gate -> buffer 0 -> D map,
+                // du_val -> buffer 1 -> aux map (the two-buffer staging of the pre-activation side output).
+                const __nv_bfloat16* u0 = e.aux_in + static_cast<int64_t>(row0) * e.ld_aux;
+                const __nv_bfloat16* u1 = e.aux_in + static_cast<int64_t>(row1) * e.ld_aux;
+#pragma unroll
+                for (int c = 0; c < BLOCK_N / 64; ++c) {
+                    const int ncol0 = n0 + c * 64;
+                    if (ncol0 >= p.N) continue;  // warpgroup-uniform
+                    uint8_t* buf0 = grp_buf;
+                    uint8_t* buf1 = grp_buf + kCdBufBytes;
+                    if (etid == 0) tma_store_wait_read<0>();
+                    named_bar_sync(bar_id, kEpiThreads);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const int col = ncol0 + j * 8 + static_cast<int>(cpair);
+                        const bool c_ok = col < p.N;  // N % 8 == 0: col and col + 1 together
+                        uint32_t xa[2] = {0, 0}, xb[2] = {0, 0};
+                        if (c_ok) {
+                            if (row0_ok) {
+                                xa[0] = __ldg(reinterpret_cast<const uint32_t*>(u0 + col));
+                                xb[0] = __ldg(reinterpret_cast<const uint32_t*>(u0 + p.N + col));
+                            }
+                            if (row1_ok) {
+                                xa[1] = __ldg(reinterpret_cast<const uint32_t*>(u1 + col));
+                                xb[1] = __ldg(reinterpret_cast<const uint32_t*>(u1 + p.N + col));
+                            }
+                        }
+                        float dg[4], dv[4];
+#pragma unroll
+                        for (int q = 0; q < 4; ++q) {
+                            const float a = (q & 1) ? bf16_hi(xa[q >> 1]) : bf16_lo(xa[q >> 1]);
+                            const float b = (q & 1) ? bf16_hi(xb[q >> 1]) : bf16_lo(xb[q >> 1]);
+                            const float dh = d[(c * 8 + j) * 4 + q];
+                            const float sg = sigmoid_approx(a);
+                            const bool ok = c_ok && ((q >> 1) ? row1_ok : row0_ok);
+                            dv[q] = ok ? dh * (a * sg) : 0.f;  // zeros keep the column sums clean
+                            dg[q] = ok ? dh * b * (sg * fmaf(a, 1.0f - sg, 1.0f)) : 0.f;
+                        }
+                        const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
+                        st_shared_b32(smem_u32(buf0) + off0, pack_bf16x2(dg[0], dg[1]));
+                        st_shared_b32(smem_u32(buf0) + off0 + 8 * 128, pack_bf16x2(dg[2], dg[3]));
+                        st_shared_b32(smem_u32(buf1) + off0, pack_bf16x2(dv[0], dv[1]));
+                        st_shared_b32(smem_u32(buf1) + off0 + 8 * 128, pack_bf16x2(dv[2], dv[3]));
+                    }
+                    fence_proxy_async_smem();
+                    named_bar_sync(bar_id, kEpiThreads);
+                    if (etid == 0) {
+                        tma_store_4d(&tmap_d, buf0, ncol0, m0, bi, bo);
                         tma_store_4d(&tmap_aux, buf1, ncol0, m0, bi, bo);
                         tma_store_commit();
                     }
-                }
-                if (e.colsum != nullptr) {
-                    // Bias gradient: column sums of the (bf16-rounded) output tile, fp32 atomics.
-                    const int ccol = etid & 63;       // column within the chunk
-                    const int rhalf = etid >> 6;      // 0/1 -> rows [0,32) / [32,64)
-                    const int jj = ccol >> 3, within = ccol & 7;
-                    float s = 0.f;
+                    if (e.colsum != nullptr) {
+                        // fc1 bias gradient: column n of du_gate -> colsum[n], of du_val -> colsum[N + n]
+                        const int ccol = etid & 63;
+                        const int rhalf = etid >> 6;
+                        const int jj = ccol >> 3, within = ccol & 7;
+                        float s0 = 0.f, s1 = 0.f;
 #pragma unroll 8
-                    for (int r = 0; r < 32; ++r) {
-                        const int rr = rhalf * 32 + r;
-                        const uint8_t* ptr = buf0 + rr * 128 + ((jj ^ (rr & 7)) * 16) + within * 2;
-                        s += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(ptr));
+                        for (int r = 0; r < 32; ++r) {
+                            const int rr = rhalf * 32 + r;
+                            const int off = rr * 128 + ((jj ^ (rr & 7)) * 16) + within * 2;
+                            s0 += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(buf0 + off));
+                            s1 += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(buf1 + off));
+                        }
+                        if (ncol0 + ccol < p.N) {
+                            atomicAdd(e.colsum + ncol0 + ccol, s0);
+                            atomicAdd(e.colsum + p.N + ncol0 + ccol, s1);
+                        }
                     }
-                    if (ncol0 + ccol < p.N)
-                        atomicAdd(e.colsum + static_cast<int64_t>(bi) * e.colsum_bi_stride + ncol0 + ccol, s);
+                    ++flip;
                 }
-                ++flip;
+            } else {
+                const __nv_bfloat16 *ext0 = nullptr, *ext1 = nullptr;
+                if (ext_is_aux) {
+                    ext0 = e.aux_in + static_cast<int64_t>(row0) * e.ld_aux;
+                    ext1 = e.aux_in + static_cast<int64_t>(row1) * e.ld_aux;
+                } else if (e.residual != nullptr) {
+                    ext0 = e.residual + static_cast<int64_t>(e.res_row_mod > 0 ? row0 % e.res_row_mod : row0) * e.ld_res;
+                    ext1 = e.residual + static_cast<int64_t>(e.res_row_mod > 0 ? row1 % e.res_row_mod : row1) * e.ld_res;
+                }
+                // kRowScale (stochastic depth): v = (acc + bias) * row_scale[row / rows_per_scale] before the residual add,
+                // the scale read once per accumulator row of the tile.  A template flag rather than a run-time branch: the
+                // GELU / dGELU epilogues run at the register limit, and any change to their code changes how ptxas
+                // schedules them; the instantiations without the flag compile exactly as they would without the feature.
+                float rs0 = 1.f, rs1 = 1.f;
+                if constexpr (kRowScale) {
+                    if (row0_ok) rs0 = __ldg(e.row_scale + row0 / e.rows_per_scale);
+                    if (row1_ok) rs1 = __ldg(e.row_scale + row1 / e.rows_per_scale);
+                }
+    #pragma unroll
+                for (int c = 0; c < BLOCK_N / 64; ++c) {
+                    const int ncol0 = n0 + c * 64;
+                    if (ncol0 >= p.N) continue;  // warpgroup-uniform: nothing to store
+                    uint8_t* buf0 = grp_buf + (e.has_aux_out ? 0 : (flip & 1)) * kCdBufBytes;
+                    uint8_t* buf1 = grp_buf + kCdBufBytes;
+                    if (etid == 0) {  // staging buffer(s) of this warpgroup free again?
+                        if (e.has_aux_out)
+                            tma_store_wait_read<0>();
+                        else
+                            tma_store_wait_read<1>();
+                    }
+                    named_bar_sync(bar_id, kEpiThreads);
+    #pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const int col = ncol0 + j * 8 + static_cast<int>(cpair);
+                        const bool c0_ok = col < p.N, c1_ok = col + 1 < p.N;
+                        float v[4] = {d[(c * 8 + j) * 4], d[(c * 8 + j) * 4 + 1], d[(c * 8 + j) * 4 + 2], d[(c * 8 + j) * 4 + 3]};
+                        uint32_t x0 = 0, x1 = 0;  // dGELU pre-activation or residual of (row0 | row1, col..col+1)
+                        if (ext0 != nullptr && c0_ok) {
+                            if (row0_ok) x0 = __ldg(reinterpret_cast<const uint32_t*>(ext0 + col));
+                            if (row1_ok) x1 = __ldg(reinterpret_cast<const uint32_t*>(ext1 + col));
+                        }
+                        if (e.bias != nullptr && c0_ok) {
+                            const uint32_t bw = __ldg(reinterpret_cast<const uint32_t*>(e.bias + col));
+                            v[0] += bf16_lo(bw), v[1] += bf16_hi(bw), v[2] += bf16_lo(bw), v[3] += bf16_hi(bw);
+                        }
+                        // 16-byte chunk j of a 128-byte row, XOR-swizzled with the row like the TMA store expects
+                        const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
+                        const uint32_t off1 = off0 + 8 * 128;  // row + 8 has the same (row & 7)
+                        if (e.has_aux_out) {
+                            st_shared_b32(smem_u32(buf1) + off0, pack_bf16x2(v[0], v[1]));
+                            st_shared_b32(smem_u32(buf1) + off1, pack_bf16x2(v[2], v[3]));
+                        }
+                        if (e.act == kActGelu) {
+    #pragma unroll
+                            for (int q = 0; q < 4; ++q) v[q] = gelu_erf(v[q]);
+                        } else if (ext_is_aux) {
+                            v[0] *= dgelu_erf(bf16_lo(x0)), v[1] *= dgelu_erf(bf16_hi(x0));
+                            v[2] *= dgelu_erf(bf16_lo(x1)), v[3] *= dgelu_erf(bf16_hi(x1));
+                        }
+                        if constexpr (kRowScale) {  // host: only with kActNone, so this is (acc + bias) * scale
+                            v[0] *= rs0, v[1] *= rs0, v[2] *= rs1, v[3] *= rs1;
+                        }
+                        if (e.residual != nullptr && !ext_is_aux) {
+                            v[0] += bf16_lo(x0), v[1] += bf16_hi(x0), v[2] += bf16_lo(x1), v[3] += bf16_hi(x1);
+                        }
+                        // rows / columns outside the problem are clipped by the TMA store; zeros keep the column sums clean
+                        if (!(row0_ok && c0_ok)) v[0] = 0.f;
+                        if (!(row0_ok && c1_ok)) v[1] = 0.f;
+                        if (!(row1_ok && c0_ok)) v[2] = 0.f;
+                        if (!(row1_ok && c1_ok)) v[3] = 0.f;
+                        st_shared_b32(smem_u32(buf0) + off0, pack_bf16x2(v[0], v[1]));
+                        st_shared_b32(smem_u32(buf0) + off1, pack_bf16x2(v[2], v[3]));
+                    }
+                    fence_proxy_async_smem();
+                    named_bar_sync(bar_id, kEpiThreads);
+                    if (etid == 0) {
+                        tma_store_4d(&tmap_d, buf0, ncol0, m0, bi, bo);
+                        tma_store_commit();
+                        if (e.has_aux_out) {
+                            tma_store_4d(&tmap_aux, buf1, ncol0, m0, bi, bo);
+                            tma_store_commit();
+                        }
+                    }
+                    if (e.colsum != nullptr) {
+                        // Bias gradient: column sums of the (bf16-rounded) output tile, fp32 atomics.
+                        const int ccol = etid & 63;       // column within the chunk
+                        const int rhalf = etid >> 6;      // 0/1 -> rows [0,32) / [32,64)
+                        const int jj = ccol >> 3, within = ccol & 7;
+                        float s = 0.f;
+    #pragma unroll 8
+                        for (int r = 0; r < 32; ++r) {
+                            const int rr = rhalf * 32 + r;
+                            const uint8_t* ptr = buf0 + rr * 128 + ((jj ^ (rr & 7)) * 16) + within * 2;
+                            s += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(ptr));
+                        }
+                        if (ncol0 + ccol < p.N)
+                            atomicAdd(e.colsum + static_cast<int64_t>(bi) * e.colsum_bi_stride + ncol0 + ccol, s);
+                    }
+                    ++flip;
+                }
             }
         }
         if (etid == 0) tma_store_wait<0>();
@@ -472,6 +645,23 @@ __global__ void __launch_bounds__(kNumThreads, 1)
         __syncwarp();
         cluster_sync();
     }
+}
+
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM, bool kRowScale>
+__global__ void __launch_bounds__(kNumThreads, 1)
+    gemm_bf16_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                          const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_aux,
+                          const KernelParams p) {
+    gemm_bf16_sm90_body<kMajorA, kMajorB, BLOCK_N, kStages, kClusterM, kRowScale, 0>(tmap_a, tmap_b, tmap_d, tmap_aux, p);
+}
+
+// SwiGLU forward (kGlu = kActSwiglu, K-major B) and fc2 dgrad (kActDSwiglu, MN-major B); A is K-major in both.
+template <int kMajorB, int BLOCK_N, int kStages, int kClusterM, int kGlu>
+__global__ void __launch_bounds__(kNumThreads, 1)
+    gemm_glu_sm90_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                         const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_aux,
+                         const KernelParams p) {
+    gemm_bf16_sm90_body<0, kMajorB, BLOCK_N, kStages, kClusterM, false, kGlu>(tmap_a, tmap_b, tmap_d, tmap_aux, p);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -574,12 +764,21 @@ void check(cudaError_t err, const char* what) {
     if (err != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(err));
 }
 
-template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM, bool kRowScale = false>
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM, bool kRowScale, int kGlu>
+constexpr auto kernel_for() {
+    if constexpr (kGlu == 0)
+        return gemm_bf16_sm90_kernel<kMajorA, kMajorB, BLOCK_N, kStages, kClusterM, kRowScale>;
+    else
+        return gemm_glu_sm90_kernel<kMajorB, BLOCK_N, kStages, kClusterM, kGlu>;
+}
+
+template <int kMajorA, int kMajorB, int BLOCK_N, int kStages, int kClusterM, bool kRowScale = false, int kGlu = 0>
 void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, const GemmOperand* aux, int M, int N,
             int K, const GemmEpilogue& epi, int max_ctas, cudaStream_t stream, const GemmAgFuse* ag) {
     constexpr int kSmem = kCdBufs * kCdBufBytes + kStages * (kBlockM + BLOCK_N) * kBlockK * 2 + 2 * kStages * 8;
     static_assert(kSmem <= 232448, "shared memory budget exceeded (227 KB per block on sm_90)");
-    auto kern = gemm_bf16_sm90_kernel<kMajorA, kMajorB, BLOCK_N, kStages, kClusterM, kRowScale>;
+    constexpr int kTileN = kGlu == kActSwiglu ? BLOCK_N / 2 : BLOCK_N;
+    auto kern = kernel_for<kMajorA, kMajorB, BLOCK_N, kStages, kClusterM, kRowScale, kGlu>();
     static bool attr_set = false;
     if (!attr_set) {
         check(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem), "cudaFuncSetAttribute");
@@ -610,10 +809,19 @@ void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, co
     // A: K-major -> (inner=K, outer=M), box (64, 128).  MN-major -> (inner=M, outer=K), box (64, 64).
     // B: K-major -> box (64, BLOCK_N / kClusterM): each CTA of a cluster loads its share.  MN-major -> box (64, 64).
     CUtensorMap ta = kMajorA == 0 ? make_tmap(A, K, M, kBlockK, kBlockM) : make_tmap(A, M, K, 64, kBlockK);
-    CUtensorMap tb =
-        kMajorB == 0 ? make_tmap(B, K, N, kBlockK, BLOCK_N / kClusterM) : make_tmap(B, N, K, 64, kBlockK);
+    // SwiGLU forward: B is the whole [2N, K] weight, read in (64, BLOCK_N / 2) gate and value boxes, and the aux output
+    // u [M, 2N] is viewed as two [M, N] halves (batch index 0 = gate, 1 = value; the second starts at column N, which
+    // is why N must be a multiple of 8).
+    CUtensorMap tb = kGlu == kActSwiglu ? make_tmap(B, K, 2 * static_cast<int64_t>(N), kBlockK, BLOCK_N / 2)
+                     : kMajorB == 0     ? make_tmap(B, K, N, kBlockK, BLOCK_N / kClusterM)
+                                        : make_tmap(B, N, K, 64, kBlockK);
     CUtensorMap td = make_tmap(D, N, M, 64, 64);
-    CUtensorMap tx = (epi.has_aux_out && aux != nullptr) ? make_tmap(*aux, N, M, 64, 64) : td;
+    CUtensorMap tx = td;
+    if (epi.has_aux_out && aux != nullptr) {
+        GemmOperand x = *aux;
+        if (kGlu == kActSwiglu) x.nb_inner = 2, x.stride_b_inner = N;
+        tx = make_tmap(x, N, M, 64, 64);
+    }
 
     KernelParams p;
     p.M = M, p.N = N, p.K = K;
@@ -621,7 +829,7 @@ void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, co
     p.nb_inner = static_cast<int>(D.nb_inner);
     p.m_tiles = (M + kBlockM - 1) / kBlockM;
     p.m_units = (p.m_tiles + kClusterM - 1) / kClusterM;
-    p.n_tiles = (N + BLOCK_N - 1) / BLOCK_N;
+    p.n_tiles = (N + kTileN - 1) / kTileN;
     p.epi = epi;
     p.n_rot = 0;
     // n-tiles per raster group: 2048 output columns.  Reasoning, not a measurement: a wave of 132 CTAs then covers
@@ -645,6 +853,42 @@ void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, co
     check(cudaGetLastError(), "gemm launch failed");
 }
 
+// SwiGLU epilogues: the checks that keep them within what the kernel implements, each named in its message.
+void gemm_glu(const GemmOperand& A, int major_a, const GemmOperand& B, int major_b, const GemmOperand& D,
+              const GemmOperand* aux_out, int M, int N, int K, const GemmEpilogue& epi, int block_n, int cluster,
+              int max_ctas, cudaStream_t stream, const GemmAgFuse* ag) {
+    const bool fwd = epi.act == kActSwiglu;
+    if (epi.residual != nullptr) throw std::runtime_error("gemm: SwiGLU epilogues take no residual");
+    if (epi.row_scale != nullptr) throw std::runtime_error("gemm: SwiGLU epilogues take no row_scale");
+    if (A.nb_inner * A.nb_outer > 1 || B.nb_inner * B.nb_outer > 1 || D.nb_inner * D.nb_outer > 1)
+        throw std::runtime_error("gemm: SwiGLU epilogues take no batched operands");
+    if (ag != nullptr && ag->world > 1) throw std::runtime_error("gemm: SwiGLU epilogues take no AG fusion");
+    if (N % 8 != 0) throw std::runtime_error("gemm: SwiGLU needs N = H' = Hd / 2 to be a multiple of 8 (Hd % 16 == 0)");
+    if (fwd) {
+        if (major_a != 0 || major_b != 0) throw std::runtime_error("gemm: SwiGLU forward needs K-major A and B");
+        if (epi.aux_in != nullptr || epi.colsum != nullptr)
+            throw std::runtime_error("gemm: SwiGLU forward takes no aux_in and no column sums");
+        if (epi.has_aux_out != (aux_out != nullptr))
+            throw std::runtime_error("gemm: SwiGLU forward: has_aux_out and the aux output go together");
+    } else {
+        if (major_a != 0 || major_b != 1) throw std::runtime_error("gemm: dSwiGLU needs K-major A and MN-major B");
+        if (epi.aux_in == nullptr || aux_out == nullptr || !epi.has_aux_out)
+            throw std::runtime_error("gemm: dSwiGLU needs aux_in (u) and an aux output (du_val)");
+        if (epi.bias != nullptr) throw std::runtime_error("gemm: dSwiGLU takes no bias");
+    }
+    if (block_n == 0) block_n = 256;
+    if (block_n != 128 && block_n != 256) throw std::runtime_error("gemm: SwiGLU block_n must be 128 or 256");
+    if (cluster == 0 || max_ctas == 1) cluster = 1;
+#define B200_GLU(MB, BN, ST, ACT)                                                                            \
+    cluster == 2 ? launch<0, MB, BN, ST, 2, false, ACT>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag) \
+                 : launch<0, MB, BN, ST, 1, false, ACT>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag)
+    if (fwd)
+        block_n == 256 ? B200_GLU(0, 256, 4, kActSwiglu) : B200_GLU(0, 128, 6, kActSwiglu);
+    else
+        block_n == 256 ? B200_GLU(1, 256, 4, kActDSwiglu) : B200_GLU(1, 128, 6, kActDSwiglu);
+#undef B200_GLU
+}
+
 }  // namespace
 
 CUtensorMap make_tensor_map_4d(const GemmOperand& op, int64_t inner, int64_t outer, int box_inner, int box_outer,
@@ -655,6 +899,10 @@ CUtensorMap make_tensor_map_4d(const GemmOperand& op, int64_t inner, int64_t out
 void gemm_bf16(const GemmOperand& A, int major_a, const GemmOperand& B, int major_b, const GemmOperand& D,
                const GemmOperand* aux_out, int M, int N, int K, const GemmEpilogue& epi, int block_n, int cluster,
                int max_ctas, cudaStream_t stream, const GemmAgFuse* ag) {
+    if (epi.act == kActSwiglu || epi.act == kActDSwiglu) {
+        gemm_glu(A, major_a, B, major_b, D, aux_out, M, N, K, epi, block_n, cluster, max_ctas, stream, ag);
+        return;
+    }
     if (N % 8 != 0 && (epi.residual || epi.aux_in))
         throw std::runtime_error("gemm: N must be a multiple of 8 when residual/aux_in are used");
     if (epi.act == kActDGelu && (epi.residual != nullptr || epi.aux_in == nullptr))

@@ -8,7 +8,17 @@
 
 namespace b200 {
 
-enum GemmAct : int { kActNone = 0, kActGelu = 1, kActDGelu = 2 };
+enum GemmAct : int { kActNone = 0, kActGelu = 1, kActDGelu = 2, kActSwiglu = 3, kActDSwiglu = 4 };
+
+// SwiGLU epilogues (timm SwiGLUPacked: u = [gate | value], g = silu(gate) * value), with N = H' = Hd / 2 output columns:
+//   kActSwiglu   forward, K-major A and B.  B is the whole [Hd, K] fc1 weight and bias the whole [Hd] fc1 bias; a tile
+//                multiplies by B rows [n, n + BLOCK_N / 2) (gate) and [H' + n, ...) (value) and writes
+//                D[m, n] = silu(a) * b, a / b the gate / value pre-activations with bias.  With an aux output (the
+//                [M, Hd] matrix u) it also stores a at u[m, n] and b at u[m, H' + n].
+//   kActDSwiglu  fc2 dgrad, K-major A, MN-major B: acc = dh[m, n]; aux_in = u [M, Hd] (a at column n, b at H' + n).
+//                Writes du_gate = dh * b * silu'(a) through D (columns [0, H') of du) and du_val = dh * silu(a) through
+//                the aux output (columns [H', Hd) of du); colsum [Hd] receives the column sums of both halves.
+// Neither takes a residual, a row scale, batched operands or AG fusion; H' must be a multiple of 8 (Hd % 16 == 0).
 
 // A strided bf16 matrix with up to two batch dimensions.  `ld` and the batch strides are in elements.
 // The *inner* (contiguous) extent and the *outer* extent are implied by the GEMM shape and the major.
@@ -22,7 +32,7 @@ struct GemmOperand {
 struct GemmEpilogue {
     const __nv_bfloat16* bias = nullptr;      // [N]           v += bias[n]
     const __nv_bfloat16* residual = nullptr;  // [M, ld_res]   v += residual[m, n]   (after activation)
-    const __nv_bfloat16* aux_in = nullptr;    // [M, ld_aux]   pre-activation for kActDGelu
+    const __nv_bfloat16* aux_in = nullptr;    // [M, ld_aux]   pre-activation for kActDGelu / kActDSwiglu
     float* colsum = nullptr;                  // [N] fp32      atomically += sum_m out[m, n]
     int64_t ld_res = 0;
     int64_t ld_aux = 0;

@@ -5,7 +5,8 @@ can rebuild a full ``state_dict`` "loadable into a plain (non-FSDP) ViT" (utils.
 ``PlainViT.load_state_dict(consolidated, strict=True)`` accepts exactly what ``consolidate_sharded_ckpts`` writes.
 The architecture is the reference's FSDPViTModel (run_vit_training.py:99-162) without the wrappers: conv patch embed,
 learned position embedding, pre-LN blocks (LayerNorm eps 1e-5, optionally on q and k per head: ``cfg.qk_norm``;
-optionally LayerScale on both branches: ``cfg.init_values``), final LayerNorm (eps 1e-6), mean pool, linear head.
+optionally LayerScale on both branches: ``cfg.init_values``; optionally a SwiGLU MLP: ``cfg.swiglu``), final
+LayerNorm (eps 1e-6), mean pool, linear head.
 With ``cfg.class_token`` it is timm's token layout instead: ``cls_token`` and ``reg_token`` in front of the patches,
 ``pos_embed`` over all tokens (or the patches only, ``cfg.no_embed_class``), and the head on token 0.
 It runs on stock PyTorch ops (any device) and is meant for evaluation / export / fine-tuning outside the engine.
@@ -54,6 +55,24 @@ class _Mlp(nn.Module):
         return self.drop(self.fc2(self.drop(self.act(self.fc1(x)))))
 
 
+class _GluMlp(nn.Module):
+    """timm GluMlp(act_layer=nn.SiLU, gate_last=False), i.e. SwiGLUPacked: fc1 -> [gate | value], silu(gate) * value,
+    drop1, norm (Identity), fc2, drop2."""
+
+    def __init__(self, dim: int, hidden: int, drop: float):
+        super().__init__()
+        self.fc1 = nn.Linear(dim, hidden)
+        self.act = nn.SiLU()
+        self.drop1 = nn.Dropout(drop)
+        self.norm = nn.Identity()
+        self.fc2 = nn.Linear(hidden // 2, dim)
+        self.drop2 = nn.Dropout(drop)
+
+    def forward(self, x):
+        gate, value = self.fc1(x).chunk(2, dim=-1)
+        return self.drop2(self.fc2(self.norm(self.drop1(self.act(gate) * value))))
+
+
 class _LayerScale(nn.Module):
     """timm LayerScale: x * gamma, gamma [dim] starting at init_values."""
 
@@ -72,7 +91,7 @@ class _Block(nn.Module):
         self.attn = _Attention(cfg.embed_dim, cfg.num_heads, cfg.att_dropout, cfg.mlp_dropout, cfg.qk_norm)
         self.ls1 = _LayerScale(cfg.embed_dim, cfg.init_values) if cfg.init_values else nn.Identity()
         self.norm2 = nn.LayerNorm(cfg.embed_dim, eps=1e-5)
-        self.mlp = _Mlp(cfg.embed_dim, cfg.hidden_dim, cfg.mlp_dropout)
+        self.mlp = (_GluMlp if cfg.swiglu else _Mlp)(cfg.embed_dim, cfg.hidden_dim, cfg.mlp_dropout)
         self.ls2 = _LayerScale(cfg.embed_dim, cfg.init_values) if cfg.init_values else nn.Identity()
 
     def forward(self, x):

@@ -3,6 +3,9 @@
 Architecture parity with the reference model (run_vit_training.py:99-162, timm 0.4.12 blocks):
   * PatchEmbed = Conv2d(3, D, k=s=P) -> tokens; learned pos_embed; dropout           (:124-129,156-157)
   * num_blocks pre-LN blocks: x += proj(attn(norm1(x))); x += fc2(gelu(fc1(norm2(x))))  (:133-141)
+    - optional SwiGLU MLP (timm SwiGLUPacked = GluMlp(act_layer=SiLU, gate_last=False), off in the reference):
+      u = fc1(norm2(x)) of width Hd = [gate | value], x += fc2(silu(u[:, :Hd/2]) * u[:, Hd/2:]); the gate runs in the
+      fc1 GEMM epilogue and its gradient in the fc2 dgrad epilogue, as GELU's do
     - LayerNorm eps 1e-5 inside blocks, qkv_bias=True, exact (erf) GELU
     - optional QK normalisation (timm Attention(qk_norm=True), off in the reference): q and k of every head go through
       LayerNorm(head_dim, eps 1e-5) (attn.q_norm / attn.k_norm, one weight and bias shared by the heads) before q k^T
@@ -48,7 +51,7 @@ FINAL_LN_EPS = 1e-6  # run_vit_training.py:151
 # Parameter inventory
 # ------------------------------------------------------------------------------------------------
 def block_param_specs(cfg: ViTConfig) -> List[Tuple[str, Tuple[int, ...]]]:
-    D, Hd, hd = cfg.embed_dim, cfg.hidden_dim, cfg.head_dim
+    D, Hd, hd, Ho = cfg.embed_dim, cfg.hidden_dim, cfg.head_dim, cfg.mlp_out_dim
     qk = [("attn.q_norm.weight", (hd,)), ("attn.q_norm.bias", (hd,)),
           ("attn.k_norm.weight", (hd,)), ("attn.k_norm.bias", (hd,))] if cfg.qk_norm else []
     ls = [("ls1.gamma", (D,)), ("ls2.gamma", (D,))] if cfg.init_values else []
@@ -60,7 +63,7 @@ def block_param_specs(cfg: ViTConfig) -> List[Tuple[str, Tuple[int, ...]]]:
         *ls[:1],  # timm's Block registers ls1 / ls2 after attn / mlp
         ("norm2.weight", (D,)), ("norm2.bias", (D,)),
         ("mlp.fc1.weight", (Hd, D)), ("mlp.fc1.bias", (Hd,)),
-        ("mlp.fc2.weight", (D, Hd)), ("mlp.fc2.bias", (D,)),
+        ("mlp.fc2.weight", (D, Ho)), ("mlp.fc2.bias", (D,)),
         *ls[1:],
     ]
 
@@ -112,7 +115,7 @@ def init_block_params(cfg: ViTConfig, gen, device="cpu") -> Dict[str, torch.Tens
     p["attn.qkv.weight"], p["attn.qkv.bias"] = _linear_init(3 * D, D, gen, device=device)
     p["attn.proj.weight"], p["attn.proj.bias"] = _linear_init(D, D, gen, device=device)
     p["mlp.fc1.weight"], p["mlp.fc1.bias"] = _linear_init(Hd, D, gen, device=device)
-    p["mlp.fc2.weight"], p["mlp.fc2.bias"] = _linear_init(D, Hd, gen, device=device)
+    p["mlp.fc2.weight"], p["mlp.fc2.bias"] = _linear_init(D, cfg.mlp_out_dim, gen, device=device)
     if cfg.qk_norm:  # nn.LayerNorm init: draws nothing, so every other parameter equals the same-seed model's
         hd = cfg.head_dim
         for n in ("q_norm", "k_norm"):
@@ -228,7 +231,8 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     With cfg.qk_norm the attention runs on qkn = qk_norm(qkv).  The lean set keeps the un-normalised qkv and the norm's
     fp32 statistics; save=True also keeps qkn (a checkpoint recompute goes straight into the backward, which needs it).
     A forward that saves nothing normalises in place.
-    With prefix tokens every image has cfg.num_tokens rows (class and register tokens first); the block is unchanged."""
+    With prefix tokens every image has cfg.num_tokens rows (class and register tokens first); the block is unchanged.
+    With cfg.swiglu, u is the packed [T, Hd] fc1 pre-activation [gate | value] and g = silu(gate) * value [T, Hd / 2]."""
     do_save = save is not False and save is not None
     if save is True:
         extras = frozenset(("P", "h", "g"))
@@ -283,11 +287,12 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
         x1 = ops.linear_fwd(a, w_proj, b_proj, residual=x, **rs_att)
     del w_proj, b_proj
     h2, m2, r2 = ops.ln_fwd(x1, p["norm2.weight"], p["norm2.bias"], BLOCK_LN_EPS)
+    act = "swiglu" if cfg.swiglu else "gelu"
     if do_save:
-        g, u = ops.linear_fwd(h2, p["mlp.fc1.weight"], p["mlp.fc1.bias"], act="gelu", want_preact=True,
+        g, u = ops.linear_fwd(h2, p["mlp.fc1.weight"], p["mlp.fc1.bias"], act=act, want_preact=True,
                               ag=ag.get("mlp.fc1.weight"))
     else:
-        g, u = ops.linear_fwd(h2, p["mlp.fc1.weight"], p["mlp.fc1.bias"], act="gelu", ag=ag.get("mlp.fc1.weight")), None
+        g, u = ops.linear_fwd(h2, p["mlp.fc1.weight"], p["mlp.fc1.bias"], act=act, ag=ag.get("mlp.fc1.weight")), None
     w_fc2, b_fc2 = _branch_layer(ops, cfg, p, "mlp.fc2", "ls2")
     if use_drop and pm > 0:
         masks["fc1"] = drop.key(site + 2)
@@ -344,7 +349,7 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
         G["mlp.fc2.bias"].copy_(s2)
     g = s.pop("g", None)
     if g is None:  # not kept: re-materialise from the pre-activation
-        g = ops.gelu_fwd(s["u"])
+        g = ops.swiglu_fwd(s["u"]) if cfg.swiglu else ops.gelu_fwd(s["u"])
         if "fc1" in masks:
             g = ops.dropout(g, pm, masks["fc1"])
     ops.linear_wgrad(dt, g, out=G["mlp.fc2.weight"])
@@ -352,8 +357,10 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     w_fc2 = _layer_scale_bwd(ops, p, G, "mlp.fc2", "ls2", s2) if cfg.init_values else p["mlp.fc2.weight"]
     if "fc1" in masks:
         dg = ops.dropout(ops.linear_dgrad(dt, w_fc2), pm, masks["fc1"])
-        du = ops.dgelu_mul(dg, s["u"])
+        du = ops.swiglu_bwd(dg, s["u"]) if cfg.swiglu else ops.dgelu_mul(dg, s["u"])
         db1 = ops.colsum(du)
+    elif cfg.swiglu:
+        du, db1 = ops.linear_dgrad(dt, w_fc2, dswiglu_preact=s["u"], want_colsum=True)
     else:
         du, db1 = ops.linear_dgrad(dt, w_fc2, dgelu_preact=s["u"], want_colsum=True)
     del w_fc2

@@ -16,6 +16,9 @@ Every function launches hand-written kernels from ``_C.so``:
   * prefix tokens: the class / register tokens put in front of every image's patch rows, and the backward that splits
     the token gradient into the patch rows and the per-token batch sums (``tokens_fwd`` / ``tokens_bwd``,
     csrc/prefix_tokens.cu).
+  * SwiGLU: the gate silu(u[:, :Hd/2]) * u[:, Hd/2:] in the fc1 GEMM epilogue and its gradient in the fc2 dgrad
+    epilogue (ACT_SWIGLU / ACT_DSWIGLU), and the memory-bound ``swiglu_fwd`` / ``swiglu_bwd`` for short K, the
+    re-materialisation of g in backward and the MLP-dropout route.
   * stochastic depth: per-sample Philox scales (``drop_path_scale``), applied as a row scale in the proj / fc2 GEMM
     epilogues, and ``drop_path_bwd`` (scaled branch gradient + its bias gradient in one pass).
 
@@ -68,13 +71,19 @@ _C = _CountingModule(native.load())
 def launch_count() -> int:
     return _C.count
 
-ACT_NONE, ACT_GELU, ACT_DGELU = 0, 1, 2
+ACT_NONE, ACT_GELU, ACT_DGELU, ACT_SWIGLU, ACT_DSWIGLU = 0, 1, 2, 3, 4
 # GELU / dGELU are fused into the GEMM epilogue only when the reduction is deep enough to hide the math
 # (ViT-10B: K = 5120 fused; ViT-L: K = 1024 -> plain GEMM + stand-alone elementwise kernel; the threshold has not
 # been re-measured on H100)
 import os as _os
 
 FUSE_ACT_MIN_K = int(_os.environ.get("B200_FUSE_ACT_MIN_K", "2048"))
+# SwiGLU routes, chosen by tools/bench_swiglu.py (H100 80GB HBM3, 700 W, 32768 rows; numbers in DESIGN.md):
+#   fc1 forward: the fused epilogue took 0.69x (K = D = 1536) and 0.89x (K = 5120) the time of GEMM + swiglu_fwd
+#   fc2 dgrad:   the fused epilogue took 0.85x at K = D = 1536 but 1.14x at K = 5120 the time of GEMM + swiglu_bwd +
+#                colsum, so it runs only for K in the measured-faster range
+SWIGLU_FWD_MIN_K = 1536
+SWIGLU_DGRAD_K = (1536, 2048)
 
 # SM carve-out for compute kernels while a communication kernel runs next to them (0 = all SMs).
 _max_ctas = 0
@@ -229,6 +238,8 @@ def linear_fwd(x, w, bias=None, act: Optional[str] = None, residual=None, res_ro
     (x w^T + bias) * row_scale[m / rows_per_scale] before the residual add; only without an activation."""
     M, K = x.shape
     N = w.shape[0]
+    if act == "swiglu":
+        return _linear_swiglu(x, w, bias, residual, want_preact, ag, row_scale)
     if row_scale is not None:
         assert act is None and not want_preact and rows_per_scale > 0, "row_scale: plain linear layers only"
         assert row_scale.dtype == torch.float32 and row_scale.numel() * rows_per_scale == M, "one scale per sample"
@@ -254,9 +265,44 @@ def linear_fwd(x, w, bias=None, act: Optional[str] = None, residual=None, res_ro
     return (y, pre) if want_preact else y
 
 
-def linear_dgrad(dy, w, dgelu_preact=None, want_colsum: bool = False):
+def _linear_swiglu(x, w, bias, residual, want_preact: bool, ag, row_scale):
+    """act="swiglu" (w: the packed [Hd, K] fc1 weight): g [M, Hd / 2], and the pre-activation u [M, Hd] if wanted.
+    The GEMM tiles pair fc1 rows n and Hd / 2 + n, so the gate runs in registers; at short K the plain GEMM and
+    ``swiglu_fwd`` run instead (SWIGLU_FWD_MIN_K)."""
+    assert residual is None and row_scale is None, "swiglu: no residual or row scale"
+    M, K = x.shape
+    Hd = w.shape[0]
+    if Hd % 16 != 0:
+        raise ValueError(f"swiglu: the fc1 width Hd must be a multiple of 16, got {Hd}")
+    if K < SWIGLU_FWD_MIN_K and ag is None:
+        pre = linear_fwd(x, w, bias)
+        g = swiglu_fwd(pre)
+        return (g, pre) if want_preact else g
+    x, w = _tma_rows(x), _tma_rows(w)
+    g = torch.empty(M, Hd // 2, dtype=x.dtype, device=x.device)
+    pre = torch.empty(M, Hd, dtype=x.dtype, device=x.device) if want_preact else None
+    gemm_raw(x, _ld(x), 0, w, _ld(w), 0, g, Hd // 2, M, Hd // 2, K, bias=bias, aux_out=pre, ld_aux_out=Hd,
+             act=ACT_SWIGLU, ag=ag or ())
+    return (g, pre) if want_preact else g
+
+
+def linear_dgrad(dy, w, dgelu_preact=None, want_colsum: bool = False, dswiglu_preact=None):
+    """dswiglu_preact = u [M, Hd]: returns du = [dh * value * silu'(gate) | dh * silu(gate)] [M, Hd] for
+    dh = dy @ w [M, Hd / 2] (like ``torch_ops.linear_dgrad``): from the fc2 dgrad epilogue where that measured faster
+    (SWIGLU_DGRAD_K over the reduction depth N = D), else the plain dgrad + ``swiglu_bwd`` + ``colsum``."""
     M, N = dy.shape
     K = w.shape[1]
+    if dswiglu_preact is not None:
+        u = dswiglu_preact
+        if not SWIGLU_DGRAD_K[0] <= N <= SWIGLU_DGRAD_K[1]:
+            du = swiglu_bwd(linear_dgrad(dy, w), u)
+            return (du, colsum(du)) if want_colsum else du
+        dy, w = _tma_rows(dy), _tma_rows(w)
+        du = torch.empty(M, 2 * K, dtype=dy.dtype, device=dy.device)
+        cs = torch.zeros(2 * K, dtype=torch.float32, device=dy.device) if want_colsum else None
+        gemm_raw(dy, _ld(dy), 0, w, _ld(w), 1, du, 2 * K, M, K, N, aux_in=u, ld_aux=_ld(u), aux_out=du[:, K:],
+                 ld_aux_out=2 * K, act=ACT_DSWIGLU, colsum=cs)
+        return (du, cs) if want_colsum else du
     if dgelu_preact is not None and N < FUSE_ACT_MIN_K and K % 8 == 0:
         dx = linear_dgrad(dy, w)
         _C.dgelu_mul(dx, dgelu_preact, dx)
@@ -291,6 +337,22 @@ def gelu_fwd(u):
 def dgelu_mul(dg, u):
     du = torch.empty_like(dg)
     _C.dgelu_mul(dg.contiguous(), u, du)
+    return du
+
+
+def swiglu_fwd(u):
+    """g [M, Hd / 2] = silu(u[:, :Hd/2]) * u[:, Hd/2:] (csrc/elementwise.cu), like ``torch_ops.swiglu_fwd``."""
+    u = u.contiguous()
+    g = torch.empty(u.shape[0], u.shape[1] // 2, dtype=u.dtype, device=u.device)
+    _C.swiglu_fwd(u, g)
+    return g
+
+
+def swiglu_bwd(dg, u):
+    """du [M, Hd] = [dg * value * silu'(gate) | dg * silu(gate)], like ``torch_ops.swiglu_bwd``."""
+    u = u.contiguous()
+    du = torch.empty_like(u)
+    _C.swiglu_bwd(dg.contiguous(), u, du)
     return du
 
 

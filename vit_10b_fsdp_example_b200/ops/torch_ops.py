@@ -157,17 +157,48 @@ def dgelu(u):
     return cdf + uf * pdf
 
 
+# ------------------------------------------------------------------------------------------------
+# SwiGLU (timm SwiGLUPacked = GluMlp(act_layer=SiLU, gate_last=False)): u = [gate | value] [T, Hd], g [T, Hd / 2]
+# ------------------------------------------------------------------------------------------------
+def _swiglu(u):
+    h = u.shape[1] // 2
+    return F.silu(u[:, :h]) * u[:, h:]
+
+
+def _dswiglu(dg, u):
+    """du = [dg * value * silu'(gate) | dg * silu(gate)] in fp32; silu'(a) = s (1 + a (1 - s)), s = sigmoid(a)."""
+    h = u.shape[1] // 2
+    a, b = u[:, :h], u[:, h:]
+    s = torch.sigmoid(a)
+    return torch.cat([dg * b * (s * (1.0 + a * (1.0 - s))), dg * (a * s)], dim=1)
+
+
+def swiglu_fwd(u):
+    """g [T, Hd / 2] = silu(u[:, :Hd/2]) * u[:, Hd/2:], computed in fp32 and rounded once."""
+    return _swiglu(_f32(u)).to(u.dtype)
+
+
+def swiglu_bwd(dg, u):
+    """du [T, Hd] = [dg * value * silu'(gate) | dg * silu(gate)], rounded to dg's dtype."""
+    return _dswiglu(_f32(dg), _f32(u)).to(dg.dtype)
+
+
 def linear_fwd(x, w, bias=None, act: Optional[str] = None, residual=None, res_row_mod: int = 0,
                want_preact: bool = False, ag=None, row_scale=None, rows_per_scale: int = 0):
     """y = act(x @ w.T + bias) + residual.  residual rows may be broadcast with period res_row_mod.
     row_scale (fp32 [M / rows_per_scale], no activation): y = (x @ w.T + bias) * row_scale[m / rows_per_scale]
-    + residual -- the per-sample scale of stochastic depth."""
+    + residual -- the per-sample scale of stochastic depth.
+    act="swiglu": w is the packed [Hd, K] fc1 weight; y = silu(u[:, :Hd/2]) * u[:, Hd/2:] [M, Hd / 2] for the
+    pre-activation u = x @ w.T + bias [M, Hd] (returned as preact); no residual or row scale."""
     y = _f32(x) @ _f32(w).t()
     if bias is not None:
         y = y + _f32(bias)
     pre = y.to(x.dtype) if want_preact else None
     if act == "gelu":
         y = gelu(y)
+    elif act == "swiglu":
+        assert residual is None and row_scale is None, "swiglu: no residual or row scale"
+        y = _swiglu(y)
     elif act is not None:
         raise ValueError(act)
     if row_scale is not None:
@@ -183,10 +214,14 @@ def linear_fwd(x, w, bias=None, act: Optional[str] = None, residual=None, res_ro
     return (y, pre) if want_preact else y
 
 
-def linear_dgrad(dy, w, dgelu_preact=None, want_colsum: bool = False):
-    """dx = dy @ w  (optionally  * gelu'(preact)); colsum(dx) is the bias grad of the layer below."""
+def linear_dgrad(dy, w, dgelu_preact=None, want_colsum: bool = False, dswiglu_preact=None):
+    """dx = dy @ w  (optionally  * gelu'(preact)); colsum(dx) is the bias grad of the layer below.
+    dswiglu_preact = u [M, Hd] (the packed fc1 pre-activation): dh = dy @ w is [M, Hd / 2] and the result is the fc1
+    output gradient du = [dh * value * silu'(gate) | dh * silu(gate)] [M, Hd], with colsum over all Hd columns."""
     dx = _f32(dy) @ _f32(w)
-    if dgelu_preact is not None:
+    if dswiglu_preact is not None:
+        dx = _dswiglu(dx, _f32(dswiglu_preact))
+    elif dgelu_preact is not None:
         dx = dx * dgelu(dgelu_preact)
     dx = dx.to(dy.dtype)
     cs = _f32(dx).sum(dim=0) if want_colsum else None

@@ -238,12 +238,16 @@ class Sm100Backend(TorchDistBackend):
 
     def fusable_params(self, layout: UnitLayout):
         """Weights whose all-gather can run inside the forward GEMM that consumes them: per-parameter shard
-        groups made of whole rows (dim-0 slabs), no padding."""
+        groups made of whole rows (dim-0 slabs), no padding.  A SwiGLU fc1 (fc2 reads half its rows) is left to the
+        unit all-gather: its GEMM tiles read a gate and a value row range, which sit in two different slabs."""
         if self.world == 1 or layout.flatten:
             return ()
+        shapes = {p.name: p.shape for p in layout.params}
+        glu = ("mlp.fc1.weight" in shapes and "mlp.fc2.weight" in shapes
+               and 2 * shapes["mlp.fc2.weight"][1] == shapes["mlp.fc1.weight"][0])
         ok = []
         for g in layout.groups:
-            if g.name not in self.FUSED_PARAMS:
+            if g.name not in self.FUSED_PARAMS or (glu and g.name == "mlp.fc1.weight"):
                 continue
             spec = next(p for p in layout.params if p.name == g.name)
             rows, cols = spec.shape

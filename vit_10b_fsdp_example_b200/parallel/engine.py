@@ -466,7 +466,8 @@ class FSDPViT:
         # no P to keep: its budget goes to the LayerNorm outputs and gelu(u) instead
         flash = bool(getattr(self.ops, "use_flash", lambda n, hd: False)(cfg.num_tokens, cfg.head_dim))
         p_bytes = 0 if flash else batch * cfg.num_heads * cfg.num_tokens * npad * es
-        return (("P", p_bytes), ("h", 2 * unit), ("g", int(cfg.mlp_ratio * unit)))
+        # g is [T, mlp_out_dim]: mlp_ratio units, or mlp_ratio / 2 with SwiGLU (the lean set's u is [T, Hd] either way)
+        return (("P", p_bytes), ("h", 2 * unit), ("g", int(cfg.mlp_out_dim / cfg.embed_dim * unit)))
 
     def _save_mode(self, i: int, keep_from: int):
         """What block i stores in forward: False = only its input (checkpoint), True = everything
@@ -674,6 +675,7 @@ class FSDPViT:
             raise ValueError("the checkpoint has ls1.gamma / ls2.gamma parameters (it was trained with LayerScale): "
                              "pass --init_values to load it (any value > 0; the learned gammas are loaded)")
         self.check_prefix_tokens(full)
+        self.check_mlp_form(full)
         for u in self.all_units:
             lay = u.layout
             prefix = "" if u is self.root else u.name + "."
@@ -689,6 +691,21 @@ class FSDPViT:
             lay.shard_from_full(buf, self.shard_rank, shard)
             self._install_master(u, shard.to(self.device))
         self.backend.params_updated()
+
+    def check_mlp_form(self, full: Dict[str, torch.Tensor]) -> None:
+        """Refuse a consolidated checkpoint whose MLP form does not match --swiglu, read from the shapes: an fc2 input
+        width equal to half the fc1 rows is SwiGLU (timm SwiGLUPacked), an equal width is the GELU MLP."""
+        key = next((k for k in full if k.endswith("mlp.fc1.weight")), None)
+        if key is None or key[: -len("fc1.weight")] + "fc2.weight" not in full:
+            return
+        rows, width = full[key].shape[0], full[key[: -len("fc1.weight")] + "fc2.weight"].shape[-1]
+        glu = 2 * width == rows
+        if self.cfg.swiglu and not glu:
+            raise ValueError(f"this model uses --swiglu, but the checkpoint's MLP is not SwiGLU ({key} has {rows} rows "
+                             f"and fc2 reads {width} features, not {rows // 2}): drop --swiglu to load it")
+        if glu and not self.cfg.swiglu:
+            raise ValueError(f"the checkpoint's MLP is SwiGLU ({key} has {rows} rows and fc2 reads half of them, "
+                             f"{width}): pass --swiglu to load it")
 
     def check_prefix_tokens(self, full: Dict[str, torch.Tensor]) -> None:
         """Refuse a consolidated checkpoint whose prefix-token layout (class token, register tokens, rows of pos_embed)
@@ -736,7 +753,7 @@ class FSDPViT:
             "patch_k": self.cfg.patch_k,
             "model": {k: getattr(self.cfg, k) for k in ("image_size", "patch_size", "embed_dim", "num_heads",
                                                         "num_blocks", "mlp_ratio", "num_classes", "class_token",
-                                                        "reg_tokens", "no_embed_class")},
+                                                        "reg_tokens", "no_embed_class", "swiglu")},
         }
 
     def __repr__(self) -> str:
