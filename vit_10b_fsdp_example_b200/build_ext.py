@@ -21,7 +21,8 @@ BUILD_DIR = os.path.join(CSRC, "build")
 SO_PATH = os.path.join(PKG_DIR, "_C.so")
 
 CU_SOURCES = ["gemm_sm90.cu", "elementwise.cu", "comm.cu", "attention_sm90.cu", "attention_drop_sm90.cu",
-              "layernorm_stream.cu", "qk_norm.cu", "layer_scale.cu", "prefix_tokens.cu"]
+              "layernorm_stream.cu", "qk_norm.cu", "layer_scale.cu", "prefix_tokens.cu",
+              "patch_drop.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 
 NVCC_FLAGS = [

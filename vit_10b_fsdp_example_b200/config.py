@@ -105,6 +105,10 @@ def build_arg_parser() -> argparse.ArgumentParser:
                         help="SwiGLU MLP (timm mlp_layer=SwiGLUPacked, act_layer=nn.SiLU; Shazeer 2020, DINOv2-g): "
                              "fc1 makes Hd = int(embed_dim * mlp_ratio) features [gate | value], fc2 reads "
                              "silu(gate) * value of width Hd / 2; Hd must be a multiple of 16")
+    parser.add_argument("--patch_drop_rate", type=_patch_drop_rate, default=0.0,
+                        help="patch dropout (timm PatchDropout; Liu et al. 2022, FLIP): in training every image keeps "
+                             "a random max(1, int(N * (1 - rate))) of its N patch tokens (the class / register tokens "
+                             "always), so every block runs on fewer tokens; evaluation keeps all; 0 = off")
     return parser
 
 
@@ -130,6 +134,13 @@ def _drop_path_rate(s: str) -> float:
     v = float(s)
     if not 0.0 <= v < 1.0:
         raise argparse.ArgumentTypeError(f"--drop_path_rate must be in [0, 1), got {s}")
+    return v
+
+
+def _patch_drop_rate(s: str) -> float:
+    v = float(s)
+    if not 0.0 <= v < 1.0:
+        raise argparse.ArgumentTypeError(f"--patch_drop_rate must be in [0, 1), got {s}")
     return v
 
 
@@ -200,6 +211,7 @@ class ViTConfig:
     reg_tokens: int = 0  # learned register tokens after the class token (needs class_token)
     no_embed_class: bool = False  # pos_embed covers the patches only (timm no_embed_class=True; needs class_token)
     swiglu: bool = False  # SwiGLU MLP (timm SwiGLUPacked): fc1 -> [gate | value] of width hidden_dim, fc2 reads half of it
+    patch_drop_rate: float = 0.0  # patch dropout in training (timm PatchDropout, ordered); 0 = off
 
     def __post_init__(self):
         if not 0.0 <= self.drop_path_rate < 1.0:
@@ -217,6 +229,8 @@ class ViTConfig:
             raise ValueError(f"init_values must be a finite number >= 0, got {self.init_values}")
         if not (isinstance(self.reg_tokens, int) and self.reg_tokens >= 0):
             raise ValueError(f"reg_tokens must be an integer >= 0, got {self.reg_tokens}")
+        if not 0.0 <= self.patch_drop_rate < 1.0:
+            raise ValueError(f"patch_drop_rate must be in [0, 1), got {self.patch_drop_rate}")
         check_prefix_flags(self)
         check_swiglu(self)
 
@@ -236,7 +250,7 @@ class ViTConfig:
                    smoothing=getattr(cfg, "smoothing", 0.0), qk_norm=getattr(cfg, "qk_norm", False),
                    init_values=getattr(cfg, "init_values", 0.0), class_token=getattr(cfg, "class_token", False),
                    reg_tokens=getattr(cfg, "reg_tokens", 0), no_embed_class=getattr(cfg, "no_embed_class", False),
-                   swiglu=getattr(cfg, "swiglu", False))
+                   swiglu=getattr(cfg, "swiglu", False), patch_drop_rate=getattr(cfg, "patch_drop_rate", 0.0))
 
     @property
     def grid(self) -> int:
@@ -256,6 +270,17 @@ class ViTConfig:
     def num_tokens(self) -> int:
         """T = N + P: the tokens per image every block runs on."""
         return self.num_patches + self.num_prefix_tokens
+
+    @property
+    def num_keep(self) -> int:
+        """K: the patches every image keeps in a training step, max(1, int(N * (1 - patch_drop_rate))) in float64 as
+        timm's PatchDropout computes it (N at rate 0)."""
+        return max(1, int(self.num_patches * (1.0 - float(self.patch_drop_rate))))
+
+    @property
+    def train_tokens(self) -> int:
+        """T' = P + K: the tokens per image every block runs on in a training step (num_tokens at rate 0)."""
+        return self.num_prefix_tokens + self.num_keep
 
     @property
     def pos_len(self) -> int:

@@ -13,6 +13,7 @@
 #include "elementwise.h"
 #include "gemm_sm90.h"
 #include "layer_scale.h"
+#include "patch_drop.h"
 #include "prefix_tokens.h"
 
 namespace {
@@ -326,6 +327,73 @@ void tokens_bwd(Tensor dx0, Tensor dpatch, Tensor dtok, int64_t B, int64_t N, in
     b200::tokens_bwd(bf16_ptr(dx0), bf16_mut(dpatch), f32_ptr(dtok), B, N, P, D, cur_stream());
 }
 
+// Patch dropout.  keep: contiguous int32 [B, K]; inv: contiguous int32 [B, N].
+void check_i32(const char* what, const char* name, const Tensor& t, int64_t rows, int64_t cols) {
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kInt && t.is_contiguous() && t.dim() == 2 && t.size(0) == rows &&
+                    t.size(1) == cols,
+                what, ": ", name, " must be a contiguous int32 CUDA tensor [", rows, ", ", cols, "]");
+}
+void patch_drop_select(Tensor keep, Tensor inv, int64_t N, int64_t K, int64_t offset, int64_t key) {
+    c10::cuda::CUDAGuard guard(keep.device());
+    const int64_t B = keep.dim() == 2 ? keep.size(0) : 0;
+    check_i32("patch_drop_select", "keep", keep, B, K);
+    check_i32("patch_drop_select", "inv", inv, B, N);
+    b200::patch_drop_select(keep.data_ptr<int>(), inv.data_ptr<int>(), B, N, K, offset, (uint64_t)key, cur_stream());
+}
+// cols: [B * K, Kpad] bf16 for the kept patches keep [B, K]; lam / box as for im2col.
+void im2col_gather(Tensor img, Tensor keep, Tensor cols, int64_t P, std::optional<double> lam,
+                   std::vector<int64_t> box) {
+    c10::cuda::CUDAGuard guard(img.device());
+    TORCH_CHECK(img.is_contiguous() && img.dim() == 4 && img.size(1) == 3, "images must be contiguous [B,3,S,S]");
+    const bool is_bf16 = img.scalar_type() == at::kBFloat16;
+    TORCH_CHECK(is_bf16 || img.scalar_type() == at::kFloat, "images must be fp32 or bf16");
+    TORCH_CHECK(keep.dim() == 2, "im2col_gather: keep must be [B, K]");
+    const int64_t B = img.size(0), K = keep.size(1);
+    check_i32("im2col_gather", "keep", keep, B, K);
+    TORCH_CHECK(cols.is_contiguous() && cols.dim() == 2 && cols.size(0) == B * K,
+                "im2col_gather: cols must be a contiguous [B * K, Kpad] matrix");
+    b200::Im2colMix mix;
+    if (lam.has_value()) {
+        TORCH_CHECK(*lam >= 0.0 && *lam <= 1.0, "im2col_gather: lam must be in [0, 1]");
+        TORCH_CHECK(box.empty() || box.size() == 4, "im2col_gather: box must be [] or [yl, yh, xl, xh]");
+        mix.lam = (float)*lam, mix.mlam = (float)(1.0 - *lam);
+        mix.mode = box.empty() ? 1 : 2;
+        if (!box.empty()) mix.yl = (int)box[0], mix.yh = (int)box[1], mix.xl = (int)box[2], mix.xh = (int)box[3];
+    } else {
+        TORCH_CHECK(box.empty(), "im2col_gather: a CutMix box needs lam");
+    }
+    b200::im2col_gather(img.data_ptr(), is_bf16, keep.data_ptr<int>(), bf16_mut(cols), (int)B, (int)img.size(2),
+                        (int)P, (int)cols.size(1), (int)K, cur_stream(), mix);
+}
+// pos: contiguous bf16 [N, D]; out: contiguous bf16 [B * K, D].
+void pos_gather(Tensor pos, Tensor keep, Tensor out) {
+    c10::cuda::CUDAGuard guard(pos.device());
+    TORCH_CHECK(pos.dim() == 2 && keep.dim() == 2, "pos_gather: pos must be [N, D] and keep [B, K]");
+    const int64_t N = pos.size(0), D = pos.size(1), B = keep.size(0), K = keep.size(1);
+    TORCH_CHECK(K >= 1 && K <= N, "pos_gather: need 1 <= K <= N, got K ", K, ", N ", N);
+    check_bf16_buf("pos_gather", "pos", pos, N * D);
+    check_i32("pos_gather", "keep", keep, B, K);
+    check_bf16_buf("pos_gather", "out", out, B * K * D);
+    b200::pos_gather(bf16_ptr(pos), keep.data_ptr<int>(), bf16_mut(out), B * K, D, cur_stream());
+}
+// dx0: contiguous bf16 [B * (P + K), D]; inv: int32 [B, N]; dpatch: bf16 [B * K, D] or None; dtok: fp32 [P + N, D].
+void patch_drop_bwd(Tensor dx0, Tensor inv, OptT dpatch, Tensor dtok, int64_t B, int64_t N, int64_t K, int64_t P) {
+    c10::cuda::CUDAGuard guard(dx0.device());
+    TORCH_CHECK(P >= 0, "patch_drop_bwd: need P >= 0 prefix tokens, got P ", P);
+    TORCH_CHECK(K >= 1 && K <= N, "patch_drop_bwd: need 1 <= K <= N, got K ", K, ", N ", N);
+    TORCH_CHECK(dx0.dim() == 2, "patch_drop_bwd: dx0 must be a [B * (P + K), D] matrix");
+    const int64_t D = dx0.size(1);
+    TORCH_CHECK(D % 8 == 0, "patch_drop_bwd: need D % 8 == 0 (16-byte vectors), got D ", D);
+    check_bf16_buf("patch_drop_bwd", "dx0", dx0, B * (P + K) * D);
+    check_i32("patch_drop_bwd", "inv", inv, B, N);
+    if (dpatch.has_value()) check_bf16_buf("patch_drop_bwd", "dpatch", *dpatch, B * K * D);
+    TORCH_CHECK(dtok.is_cuda() && dtok.scalar_type() == at::kFloat && dtok.is_contiguous() &&
+                    dtok.numel() == (P + N) * D,
+                "patch_drop_bwd: dtok must be a contiguous fp32 CUDA tensor with (P + N) * D elements");
+    b200::patch_drop_bwd(bf16_ptr(dx0), inv.data_ptr<int>(), dpatch.has_value() ? bf16_mut(*dpatch) : nullptr,
+                         f32_ptr(dtok), B, N, K, P, D, cur_stream());
+}
+
 void colsum(Tensor x, Tensor out) {
     c10::cuda::CUDAGuard guard(x.device());
     const int C = (int)x.size(-1);
@@ -505,6 +573,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("layer_scale_bwd", &layer_scale_bwd);
     m.def("tokens_fwd", &tokens_fwd);
     m.def("tokens_bwd", &tokens_bwd);
+    m.def("patch_drop_select", &patch_drop_select);
+    m.def("im2col_gather", &im2col_gather, py::arg("img"), py::arg("keep"), py::arg("cols"), py::arg("P"),
+          py::arg("lam") = py::none(), py::arg("box") = std::vector<int64_t>{});
+    m.def("pos_gather", &pos_gather);
+    m.def("patch_drop_bwd", &patch_drop_bwd);
     m.def("colsum", &colsum);
     m.def("sumsq", &sumsq);
     m.def("adamw_split", &adamw_split);

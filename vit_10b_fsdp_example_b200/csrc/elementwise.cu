@@ -21,6 +21,7 @@
 
 #include "dropout.cuh"
 #include "elementwise.h"
+#include "im2col_pixel.cuh"
 #include "ptx.cuh"
 
 namespace b200 {
@@ -1005,26 +1006,7 @@ __global__ void im2col_kernel(const T* __restrict__ img, __nv_bfloat16* __restri
         const int k = static_cast<int>(i % Kpad);
         const int64_t patch = i / Kpad;
         float v = 0.f;
-        if (k < K) {
-            const int c = k / (P * P), rem = k % (P * P), py = rem / P, px = rem % P;
-            const int gx = static_cast<int>(patch % G), gy = static_cast<int>((patch / G) % G);
-            const int64_t b = patch / (G * G);
-            if constexpr (MIX == 0) {
-                v = static_cast<float>(img[((b * 3 + c) * S + gy * P + py) * S + gx * P + px]);
-            } else {
-                const int y = gy * P + py, x = gx * P + px;
-                const int64_t pix = (static_cast<int64_t>(c) * S + y) * S + x, img_elems = 3LL * S * S;
-                const int64_t b2 = B - 1 - b;
-                if constexpr (MIX == 1) {
-                    const float a = static_cast<float>(img[b * img_elems + pix]);
-                    const float o = static_cast<float>(img[b2 * img_elems + pix]);
-                    v = __fadd_rn(__fmul_rn(a, mix.lam), __fmul_rn(o, mix.mlam));
-                } else {
-                    const bool in_box = y >= mix.yl && y < mix.yh && x >= mix.xl && x < mix.xh;
-                    v = static_cast<float>(img[(in_box ? b2 : b) * img_elems + pix]);
-                }
-            }
-        }
+        if (k < K) v = im2col_pixel<T, MIX>(img, B, S, P, G, patch, k, mix);
         cols[i] = __float2bfloat16(v);
     }
 }

@@ -9,6 +9,7 @@ optionally LayerScale on both branches: ``cfg.init_values``; optionally a SwiGLU
 LayerNorm (eps 1e-6), mean pool, linear head.
 With ``cfg.class_token`` it is timm's token layout instead: ``cls_token`` and ``reg_token`` in front of the patches,
 ``pos_embed`` over all tokens (or the patches only, ``cfg.no_embed_class``), and the head on token 0.
+With ``cfg.patch_drop_rate`` it applies timm's ``PatchDropout(ordered=True)`` after ``pos_drop`` in training.
 It runs on stock PyTorch ops (any device) and is meant for evaluation / export / fine-tuning outside the engine.
 """
 from __future__ import annotations
@@ -108,6 +109,28 @@ class _PatchEmbed(nn.Module):
         return self.proj(x).flatten(2).transpose(1, 2)
 
 
+class _PatchDropout(nn.Module):
+    """timm PatchDropout(prob, num_prefix_tokens, ordered=True): in training every image keeps
+    K = max(1, int(N * (1 - prob))) of its N patch tokens, in ascending order, and all prefix tokens.  ``keep`` [B, K]
+    pins the subset (the default draws timm's random one)."""
+
+    def __init__(self, prob: float, num_prefix_tokens: int):
+        super().__init__()
+        self.prob, self.num_prefix_tokens = prob, num_prefix_tokens
+
+    def forward(self, x, keep=None):
+        if not self.training or self.prob == 0.0:
+            return x
+        P = self.num_prefix_tokens
+        prefix, x = x[:, :P], x[:, P:]
+        B, L = x.shape[:2]
+        if keep is None:
+            num_keep = max(1, int(L * (1.0 - self.prob)))
+            keep = torch.argsort(torch.randn(B, L, device=x.device), dim=-1)[:, :num_keep].sort(dim=-1)[0]
+        x = x.gather(1, keep.long().unsqueeze(-1).expand(-1, -1, x.shape[-1]))
+        return torch.cat((prefix, x), dim=1) if P else x
+
+
 class PlainViT(nn.Module):
     def __init__(self, cfg: ViTConfig):
         super().__init__()
@@ -118,13 +141,15 @@ class PlainViT(nn.Module):
         self.reg_token = nn.Parameter(torch.zeros(1, cfg.reg_tokens, D)) if cfg.class_token and cfg.reg_tokens else None
         self.pos_embed = nn.Parameter(torch.zeros(1, cfg.pos_len, D))
         self.pos_drop = nn.Dropout(cfg.pos_dropout)
+        self.patch_drop = _PatchDropout(cfg.patch_drop_rate, cfg.num_prefix_tokens)
         self.blocks = nn.Sequential(*[_Block(cfg) for _ in range(cfg.num_blocks)])
         self.norm = nn.LayerNorm(cfg.embed_dim, eps=1e-6)
         self.head = nn.Linear(cfg.embed_dim, cfg.num_classes)
 
-    def forward(self, image):
+    def forward(self, image, patch_keep=None):
+        """patch_keep: optional [B, K] kept patches of the patch dropout (training only)."""
         if self.cls_token is None:
-            x = self.pos_drop(self.patch_embed(image) + self.pos_embed)
+            x = self.patch_drop(self.pos_drop(self.patch_embed(image) + self.pos_embed), patch_keep)
             x = self.blocks(x)
             return self.head(self.norm(x).mean(dim=1))
         x = self.patch_embed(image)
@@ -135,7 +160,7 @@ class PlainViT(nn.Module):
             x = torch.cat(prefix + [x + self.pos_embed], dim=1)
         else:
             x = torch.cat(prefix + [x], dim=1) + self.pos_embed
-        x = self.blocks(self.pos_drop(x))
+        x = self.blocks(self.patch_drop(self.pos_drop(x), patch_keep))
         return self.head(self.norm(x)[:, 0])
 
     @classmethod

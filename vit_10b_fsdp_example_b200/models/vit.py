@@ -23,6 +23,10 @@ Architecture parity with the reference model (run_vit_training.py:99-162, timm 0
     cls_token and R reg_tokens in front of every image's N patch tokens, T = N + P tokens with P = 1 + R; pos_embed
     covers all T tokens, or only the patches with no_embed_class.  The patch GEMM still adds the patch rows of pos_embed
     in its epilogue; ops.tokens_fwd / tokens_bwd assemble and split the [B*T, D] token buffer
+  * optional patch dropout (timm PatchDropout(prob=R, num_prefix_tokens=P, ordered=True), off in the reference): in
+    training every image keeps K = max(1, int(N * (1 - R))) of its patches, drawn on the GPU (ops.patch_drop_select);
+    only they go through the im2col and the patch GEMM, with their own pos_embed rows, and every block runs on
+    T' = P + K tokens.  Evaluation keeps all patches
   * final LayerNorm(eps=1e-6), mean-pool over tokens (no CLS token), Linear head      (:151-153,159-161);
     with a class token: LayerNorm of the B class rows only (it acts per row) and the head on them
 Parameter names are timm-compatible (``norm1.weight``, ``attn.qkv.weight``, ``mlp.fc1.bias`` ...).
@@ -232,6 +236,7 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     fp32 statistics; save=True also keeps qkn (a checkpoint recompute goes straight into the backward, which needs it).
     A forward that saves nothing normalises in place.
     With prefix tokens every image has cfg.num_tokens rows (class and register tokens first); the block is unchanged.
+    The tokens per image are x.shape[0] // B: T' = P + K in a training step with patch dropout.
     With cfg.swiglu, u is the packed [T, Hd] fc1 pre-activation [gate | value] and g = silu(gate) * value [T, Hd / 2]."""
     do_save = save is not False and save is not None
     if save is True:
@@ -240,7 +245,7 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
         extras = frozenset()
     else:
         extras = frozenset(save)
-    N, H, hd = cfg.num_tokens, cfg.num_heads, cfg.head_dim
+    N, H, hd = x.shape[0] // B, cfg.num_heads, cfg.head_dim
     pa, pm = cfg.att_dropout, cfg.mlp_dropout
     use_drop = drop is not None and drop.training and (pa > 0 or pm > 0)
     site = block_idx * 8
@@ -331,7 +336,7 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     ``ops.layer_scale_bwd`` rescales its result and yields the bias and gamma gradients, and the dgrad uses the
     folded weight.
     """
-    N, H, hd = cfg.num_tokens, cfg.num_heads, cfg.head_dim
+    N, H, hd = s["x"].shape[0] // B, cfg.num_heads, cfg.head_dim
     pa, pm = cfg.att_dropout, cfg.mlp_dropout
     masks = s["masks"]
     dpath = s.get("dpath")  # stochastic depth: per-sample scales of the (attention, MLP) branches, or None
@@ -462,30 +467,58 @@ def _qk_norm(ops, cfg: ViTConfig, p, qkv, inplace: bool):
 def stem_forward(ops, cfg: ViTConfig, p, images, dtype, drop: Optional[DropoutCtx] = None, mix: Optional[Mix] = None):
     """mix: this step's batch mixing (``draw_mix``), applied inside the im2col; the saved cols are the mixed patches.
     With a class token the patch GEMM adds the patch rows of pos_embed and ops.tokens_fwd puts the prefix tokens in
-    front of every image: timm's cat(prefix, patches) + pos, or cat(prefix, patches + pos) with no_embed_class."""
+    front of every image: timm's cat(prefix, patches) + pos, or cat(prefix, patches + pos) with no_embed_class.
+    With patch dropout in training (``_stem_forward_patch_drop``) every image keeps cfg.num_keep patches."""
     B = images.shape[0]
-    if mix is None:
-        cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype)
+    if drop is not None and drop.training and cfg.patch_drop_rate > 0:
+        x0, saved = _stem_forward_patch_drop(ops, cfg, p, images, dtype, drop, mix)
     else:
-        cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype, mix=mix)
-    if cfg.class_token:
-        P, pos = cfg.num_prefix_tokens, p["pos_embed"]
-        y = ops.linear_fwd(cols, p["patch_embed.proj.weight"], p["patch_embed.proj.bias"],
-                           residual=pos if cfg.no_embed_class else pos[P:], res_row_mod=cfg.num_patches)
-        x0 = ops.tokens_fwd(y, p["cls_token"], p.get("reg_token"), None if cfg.no_embed_class else pos[:P], B,
-                            cfg.num_patches)
-        del y
-    else:
-        x0 = ops.linear_fwd(cols, p["patch_embed.proj.weight"], p["patch_embed.proj.bias"], residual=p["pos_embed"],
-                            res_row_mod=cfg.num_patches)
+        if mix is None:
+            cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype)
+        else:
+            cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype, mix=mix)
+        if cfg.class_token:
+            P, pos = cfg.num_prefix_tokens, p["pos_embed"]
+            y = ops.linear_fwd(cols, p["patch_embed.proj.weight"], p["patch_embed.proj.bias"],
+                               residual=pos if cfg.no_embed_class else pos[P:], res_row_mod=cfg.num_patches)
+            x0 = ops.tokens_fwd(y, p["cls_token"], p.get("reg_token"), None if cfg.no_embed_class else pos[:P], B,
+                                cfg.num_patches)
+            del y
+        else:
+            x0 = ops.linear_fwd(cols, p["patch_embed.proj.weight"], p["patch_embed.proj.bias"],
+                                residual=p["pos_embed"], res_row_mod=cfg.num_patches)
+        saved = dict(cols=cols)
     mask = None  # dropout key of the position-embedding dropout (reference :129,157)
     if drop is not None and drop.training and cfg.pos_dropout > 0:
         mask = drop.key(7_000_001)
         x0 = ops.dropout(x0, cfg.pos_dropout, mask)
-    return x0, dict(cols=cols, mask=mask, B=B)
+    return x0, dict(saved, mask=mask, B=B)
+
+
+def _stem_forward_patch_drop(ops, cfg: ViTConfig, p, images, dtype, drop: DropoutCtx, mix: Optional[Mix]):
+    """timm PatchDropout(ordered=True) after the position embedding: image g = drop.sample_offset + b keeps the
+    patches ops.patch_drop_select draws for it (key 7_000_002), in ascending order.  Only the kept patches go through
+    the im2col and the patch GEMM, which adds the bias and their own pos_embed rows (ops.pos_gather) as its residual;
+    the prefix tokens are always kept.  pos_drop then acts on the compacted [B * (P + K), D] buffer."""
+    B, N, K, P = images.shape[0], cfg.num_patches, cfg.num_keep, cfg.num_prefix_tokens
+    keep, inv = ops.patch_drop_select(drop.key(7_000_002), B, N, K, drop.sample_offset, images.device)
+    if mix is None:
+        cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype, keep=keep)
+    else:
+        cols = ops.patch_im2col(images, cfg.patch_size, cfg.patch_kpad, dtype, mix=mix, keep=keep)
+    pos = p["pos_embed"]
+    pos_patch = pos[P:] if cfg.class_token and not cfg.no_embed_class else pos
+    x0 = ops.linear_fwd(cols, p["patch_embed.proj.weight"], p["patch_embed.proj.bias"],
+                        residual=ops.pos_gather(pos_patch, keep))
+    if cfg.class_token:
+        x0 = ops.tokens_fwd(x0, p["cls_token"], p.get("reg_token"), None if cfg.no_embed_class else pos[:P], B, K)
+    return x0, dict(cols=cols, keep=keep, inv=inv)
 
 
 def stem_backward(ops, cfg: ViTConfig, p, G, s, dx0, dx0_colsum):
+    if s.get("inv") is not None:
+        _stem_backward_patch_drop(ops, cfg, G, s, dx0)
+        return
     if cfg.class_token:
         _stem_backward_prefix(ops, cfg, G, s, dx0)
         return
@@ -495,6 +528,24 @@ def stem_backward(ops, cfg: ViTConfig, p, G, s, dx0, dx0_colsum):
     ops.linear_wgrad(dx0, s["cols"], out=G["patch_embed.proj.weight"])
     G["patch_embed.proj.bias"].copy_(dx0_colsum)
     G["pos_embed"].copy_(dx0.view(s["B"], cfg.num_patches, cfg.embed_dim).sum(dim=0, dtype=torch.float32))
+
+
+def _stem_backward_patch_drop(ops, cfg: ViTConfig, G, s, dx0):
+    """With patch dropout: one pass (ops.patch_drop_bwd) scatters dx0 [B * (P + K), D] back to the full sequence as
+    per-token batch sums dtok [P + N, D] (a dropped patch gets nothing from that image) and, with prefix tokens, copies
+    the patch rows out as the wgrad operand; without them dx0 itself is that operand."""
+    if s["mask"] is not None:
+        dx0 = ops.dropout(dx0, cfg.pos_dropout, s["mask"])
+    P = cfg.num_prefix_tokens
+    dpatch, dtok = ops.patch_drop_bwd(dx0, s["inv"], s["B"], cfg.num_patches, cfg.num_keep, P)
+    ops.linear_wgrad(dpatch if P else dx0, s["cols"], out=G["patch_embed.proj.weight"])
+    del dpatch
+    G["patch_embed.proj.bias"].copy_(dtok[P:].sum(dim=0))
+    G["pos_embed"].copy_(dtok[P:] if cfg.no_embed_class else dtok)
+    if cfg.class_token:
+        G["cls_token"].copy_(dtok[:1])
+        if cfg.reg_tokens:
+            G["reg_token"].copy_(dtok[1:P])
 
 
 def _stem_backward_prefix(ops, cfg: ViTConfig, G, s, dx0):
@@ -517,20 +568,20 @@ def _stem_backward_prefix(ops, cfg: ViTConfig, G, s, dx0):
 def head_forward(ops, cfg: ViTConfig, p, x, B: int):
     """logits = head(mean_tokens(norm(x)))   (run_vit_training.py:161)
     With a class token: logits = head(norm(x)[:, 0]); the norm acts per row, so only the B class rows are normalised."""
+    T = x.shape[0] // B  # cfg.num_tokens, or P + K in a training step with patch dropout
     if cfg.class_token:
-        xc = x.view(B, cfg.num_tokens, cfg.embed_dim)[:, 0].contiguous()
+        xc = x.view(B, T, cfg.embed_dim)[:, 0].contiguous()
         xn, m, r = ops.ln_fwd(xc, p["norm.weight"], p["norm.bias"], FINAL_LN_EPS)
         logits = ops.linear_fwd(xn, p["head.weight"], p["head.bias"])
-        return logits, dict(x=xc, m=m, r=r, pooled=xn)
-    N, D = cfg.num_patches, cfg.embed_dim
+        return logits, dict(x=xc, m=m, r=r, pooled=xn, T=T)
     xn, m, r = ops.ln_fwd(x, p["norm.weight"], p["norm.bias"], FINAL_LN_EPS)
-    pooled = ops.mean_pool(xn, B, N)
+    pooled = ops.mean_pool(xn, B, T)  # the mean over the patches present: timm's x[:, P:].mean(1) with P = 0
     logits = ops.linear_fwd(pooled, p["head.weight"], p["head.bias"])
     return logits, dict(x=x, m=m, r=r, pooled=pooled)
 
 
 def head_backward(ops, cfg: ViTConfig, p, G, s, dlogits, B: int):
-    N, D = cfg.num_patches, cfg.embed_dim
+    D = cfg.embed_dim
     ops.linear_wgrad(dlogits, s["pooled"], out=G["head.weight"])
     G["head.bias"].copy_(dlogits.sum(dim=0, dtype=torch.float32))
     dpooled = ops.linear_dgrad(dlogits, p["head.weight"])
@@ -538,10 +589,10 @@ def head_backward(ops, cfg: ViTConfig, p, G, s, dlogits, B: int):
         dxc, dnw, dnb, dx_sum = ops.ln_bwd(dpooled, s["x"], p["norm.weight"], s["m"], s["r"], want_dxsum=True)
         G["norm.weight"].copy_(dnw)
         G["norm.bias"].copy_(dnb)
-        dx = torch.zeros(B * cfg.num_tokens, D, dtype=dxc.dtype, device=dxc.device)
-        dx.view(B, cfg.num_tokens, D)[:, 0] = dxc
+        dx = torch.zeros(B * s["T"], D, dtype=dxc.dtype, device=dxc.device)
+        dx.view(B, s["T"], D)[:, 0] = dxc
         return dx, dx_sum
-    dxn = ops.mean_pool_bwd(dpooled, B, N)
+    dxn = ops.mean_pool_bwd(dpooled, B, s["x"].shape[0] // B)
     dx, dnw, dnb, dx_sum = ops.ln_bwd(dxn, s["x"], p["norm.weight"], s["m"], s["r"], want_dxsum=True)
     G["norm.weight"].copy_(dnw)
     G["norm.bias"].copy_(dnb)

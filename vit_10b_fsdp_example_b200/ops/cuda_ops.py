@@ -19,6 +19,9 @@ Every function launches hand-written kernels from ``_C.so``:
   * SwiGLU: the gate silu(u[:, :Hd/2]) * u[:, Hd/2:] in the fc1 GEMM epilogue and its gradient in the fc2 dgrad
     epilogue (ACT_SWIGLU / ACT_DSWIGLU), and the memory-bound ``swiglu_fwd`` / ``swiglu_bwd`` for short K, the
     re-materialisation of g in backward and the MLP-dropout route.
+  * patch dropout: the per-image kept-patch selection, the im2col of the kept patches, their position rows and the
+    backward of the kept-token assembly (``patch_drop_select`` / ``patch_im2col(keep=)`` / ``pos_gather`` /
+    ``patch_drop_bwd``, csrc/patch_drop.cu).
   * stochastic depth: per-sample Philox scales (``drop_path_scale``), applied as a row scale in the proj / fc2 GEMM
     epilogues, and ``drop_path_bwd`` (scaled branch gradient + its bias gradient in one pass).
 
@@ -224,6 +227,34 @@ def tokens_bwd(dx0, B: int, N: int, P: int):
     dpatch = torch.empty(B * N, D, dtype=dx0.dtype, device=dx0.device)
     dtok = torch.empty(N + P, D, dtype=torch.float32, device=dx0.device)
     _C.tokens_bwd(dx0, dpatch, dtok, B, N, P)
+    return dpatch, dtok
+
+
+# ------------------------------------------------------------------------------------------------
+# Patch dropout (csrc/patch_drop.cu): every image keeps K of its N patches in a training step
+# ------------------------------------------------------------------------------------------------
+def patch_drop_select(key: int, B: int, N: int, K: int, offset: int, device):
+    """(keep int32 [B, K], inv int32 [B, N]) with the bits of ``torch_ops.patch_drop_select``."""
+    keep = torch.empty(B, K, dtype=torch.int32, device=device)
+    inv = torch.empty(B, N, dtype=torch.int32, device=device)
+    _C.patch_drop_select(keep, inv, int(N), int(K), int(offset), _drop_key(key))
+    return keep, inv
+
+
+def pos_gather(pos, keep):
+    """[B * K, D]: the position rows pos[keep[b, i]] of the kept patches."""
+    out = torch.empty(keep.numel(), pos.shape[1], dtype=pos.dtype, device=pos.device)
+    _C.pos_gather(pos.contiguous(), keep, out)
+    return out
+
+
+def patch_drop_bwd(dx0, inv, B: int, N: int, K: int, P: int):
+    """(dpatch [B * K, D] bf16 or None when P == 0, dtok [P + N, D] fp32) in one pass, like
+    ``torch_ops.patch_drop_bwd``; dtok is summed over the batch in a fixed order (the same bits in every run)."""
+    D = dx0.shape[1]
+    dpatch = torch.empty(B * K, D, dtype=dx0.dtype, device=dx0.device) if P else None
+    dtok = torch.empty(P + N, D, dtype=torch.float32, device=dx0.device)
+    _C.patch_drop_bwd(dx0, inv, dpatch, dtok, B, N, K, P)
     return dpatch, dtok
 
 
@@ -550,10 +581,19 @@ def attention_bwd(dout, qkv, p, B: int, N: int, H: int, hd: int, want_colsum: bo
 # ------------------------------------------------------------------------------------------------
 # Patch embedding, loss
 # ------------------------------------------------------------------------------------------------
-def patch_im2col(images, P: int, kpad: int, dtype, mix=None):
+def patch_im2col(images, P: int, kpad: int, dtype, mix=None, keep=None):
     """mix = (lam, box) from vit.draw_mix: Mixup (box None) or CutMix of image b with image B-1-b, fused into the
-    im2col (torch_ops.mix_images is the reference)."""
+    im2col (torch_ops.mix_images is the reference).  keep [B, K] (patch dropout): only the kept patches, by the
+    gathering im2col kernel."""
     B, _, S, _ = images.shape
+    if keep is not None:
+        cols = torch.empty(keep.numel(), kpad, dtype=dtype, device=images.device)
+        if mix is None:
+            _C.im2col_gather(images.contiguous(), keep, cols, P)
+        else:
+            lam, box = mix
+            _C.im2col_gather(images.contiguous(), keep, cols, P, float(lam), list(box) if box is not None else [])
+        return cols
     G = S // P
     cols = torch.empty(B * G * G, kpad, dtype=dtype, device=images.device)
     if mix is None:

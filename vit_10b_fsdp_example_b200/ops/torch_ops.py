@@ -313,6 +313,55 @@ def drop_path_bwd(dy, scale, N: int):
     return dt, _f32(dt).sum(dim=0)
 
 
+# ------------------------------------------------------------------------------------------------
+# Patch dropout (timm PatchDropout(ordered=True)): the same selection bits as csrc/patch_drop.cu
+# ------------------------------------------------------------------------------------------------
+def patch_drop_keep(key: int, B: int, N: int, K: int, offset: int) -> np.ndarray:
+    """int64 [B, K]: the patches image g = offset + b keeps, ascending.  Patch n draws r = word n % 4 of
+    philox4x32_10(n / 4, g, key); the kept patches are the K smallest (r, n) pairs (a stable argsort of r)."""
+    if not 1 <= K <= N:
+        raise ValueError(f"patch dropout keeps 1 <= K <= N patches, got K {K}, N {N}")
+    key = int(key) & 0x7FFFFFFFFFFFFFFF
+    n = np.arange(N, dtype=np.uint64)
+    g = np.arange(offset, offset + B, dtype=np.uint64)
+    c0 = np.broadcast_to(n // np.uint64(4), (B, N))
+    c1 = np.broadcast_to(g[:, None], (B, N))
+    r = np.stack(philox4x32_10(c0, c1, key & 0xFFFFFFFF, key >> 32))  # [4, B, N]
+    word = r[(n % np.uint64(4)).astype(np.int64)[None, :], np.arange(B)[:, None], np.arange(N)[None, :]]  # [B, N]
+    order = np.argsort(word, axis=1, kind="stable")[:, :K]
+    return np.sort(order, axis=1)
+
+
+def patch_drop_select(key: int, B: int, N: int, K: int, offset: int, device):
+    """(keep int32 [B, K], inv int32 [B, N]): keep as ``patch_drop_keep``; inv[b, n] = row of patch n in keep[b], or
+    -1 when image b drops patch n."""
+    keep = patch_drop_keep(key, B, N, K, offset)
+    inv = np.full((B, N), -1, dtype=np.int32)
+    np.put_along_axis(inv, keep, np.arange(K, dtype=np.int32)[None, :].repeat(B, 0), axis=1)
+    return torch.from_numpy(keep.astype(np.int32)).to(device), torch.from_numpy(inv).to(device)
+
+
+def pos_gather(pos, keep):
+    """[B * K, D]: row b * K + i is pos[keep[b, i]] (the position rows of the kept patches)."""
+    return pos[keep.reshape(-1).long()].contiguous()
+
+
+def patch_drop_bwd(dx0, inv, B: int, N: int, K: int, P: int):
+    """(dpatch, dtok) for dx0 [B * (P + K), D]: dpatch [B * K, D] = the patch rows (None when P == 0: dx0 itself is
+    then the patch matrix); dtok [P + N, D] fp32, dtok[j < P] = sum_b dx0[b, j], dtok[P + n] = sum over the images that
+    kept patch n of dx0[b, P + inv[b, n]], summed in b order."""
+    D = dx0.shape[1]
+    x = dx0.reshape(B, P + K, D)
+    dtok = torch.zeros(P + N, D, dtype=torch.float32, device=dx0.device)
+    dtok[:P] = x[:, :P].sum(dim=0, dtype=torch.float32)
+    invl = inv.long()
+    for b in range(B):
+        kept = invl[b] >= 0
+        dtok[P:][kept] += _f32(x[b, P:][invl[b][kept]])
+    dpatch = x[:, P:].reshape(B * K, D).contiguous() if P else None
+    return dpatch, dtok
+
+
 def mean_pool(xn, B: int, N: int):
     """[B*N, D] -> [B, D]: mean over the tokens of an image (run_vit_training.py:161)."""
     return xn.view(B, N, -1).mean(dim=1, dtype=torch.float32).to(xn.dtype)
@@ -426,13 +475,17 @@ def mix_images(images, mix):
     return x
 
 
-def patch_im2col(images, P: int, kpad: int, dtype, mix=None):
+def patch_im2col(images, P: int, kpad: int, dtype, mix=None, keep=None):
+    """keep [B, K] (patch dropout): only the kept patches, row b * K + i = patch keep[b, i] of image b."""
     if mix is not None:
         images = mix_images(images, mix)
     B, C, S, _ = images.shape
     G = S // P
-    cols = images.view(B, C, G, P, G, P).permute(0, 2, 4, 1, 3, 5).reshape(B * G * G, C * P * P)
-    out = torch.zeros(B * G * G, kpad, dtype=dtype, device=images.device)
+    cols = images.view(B, C, G, P, G, P).permute(0, 2, 4, 1, 3, 5).reshape(B, G * G, C * P * P)
+    if keep is not None:
+        cols = torch.gather(cols, 1, keep.long()[:, :, None].expand(-1, -1, C * P * P))
+    cols = cols.reshape(-1, C * P * P)
+    out = torch.zeros(cols.shape[0], kpad, dtype=dtype, device=images.device)
     out[:, : C * P * P] = cols.to(dtype)
     return out
 

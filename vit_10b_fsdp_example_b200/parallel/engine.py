@@ -418,12 +418,13 @@ class FSDPViT:
         """HBM a block's lean activation set occupies: x, qkv (3), attention out, x1, fc1 pre-activation.  With QK
         normalisation the set keeps the un-normalised qkv plus the norm's fp32 mean and rstd per (token, q or k, head):
         16 bytes per token and head (16.8 MB per ViT-10B block at 128 images, against about 3.4 GB for the rest).
-        Every image has cfg.num_tokens rows (prefix tokens included)."""
+        Every image has cfg.train_tokens rows in a training step (prefix tokens included, dropped patches not)."""
         cfg = self.cfg
+        T = cfg.train_tokens
         units = 6.0 + cfg.mlp_ratio
-        n = int(batch * cfg.num_tokens * cfg.embed_dim * units * torch.empty((), dtype=self.dtype).element_size())
+        n = int(batch * T * cfg.embed_dim * units * torch.empty((), dtype=self.dtype).element_size())
         if cfg.qk_norm:
-            n += 16 * batch * cfg.num_tokens * cfg.num_heads
+            n += 16 * batch * T * cfg.num_heads
         return n
 
     def _auto_keep_blocks(self, batch: int) -> int:
@@ -460,12 +461,13 @@ class FSDPViT:
     def extra_bytes_per_block(self, batch: int):
         cfg = self.cfg
         es = torch.empty((), dtype=self.dtype).element_size()
-        unit = batch * cfg.num_tokens * cfg.embed_dim * es
-        npad = (cfg.num_tokens + 7) // 8 * 8
+        T = cfg.train_tokens  # tokens per image in a training step
+        unit = batch * T * cfg.embed_dim * es
+        npad = (T + 7) // 8 * 8
         # with the fused attention pair (forward keeps the row log-sum-exp, backward rebuilds P tile by tile) there is
         # no P to keep: its budget goes to the LayerNorm outputs and gelu(u) instead
-        flash = bool(getattr(self.ops, "use_flash", lambda n, hd: False)(cfg.num_tokens, cfg.head_dim))
-        p_bytes = 0 if flash else batch * cfg.num_heads * cfg.num_tokens * npad * es
+        flash = bool(getattr(self.ops, "use_flash", lambda n, hd: False)(T, cfg.head_dim))
+        p_bytes = 0 if flash else batch * cfg.num_heads * T * npad * es
         # g is [T, mlp_out_dim]: mlp_ratio units, or mlp_ratio / 2 with SwiGLU (the lean set's u is [T, Hd] either way)
         return (("P", p_bytes), ("h", 2 * unit), ("g", int(cfg.mlp_out_dim / cfg.embed_dim * unit)))
 

@@ -30,6 +30,9 @@ class GraphedTrainStep:
         if model.training and cfg.drop_path_rate > 0:
             raise RuntimeError("CUDA-graph training steps do not support drop_path_rate > 0 "
                                "(masks are keyed from the host)")
+        if model.training and cfg.patch_drop_rate > 0:
+            raise RuntimeError("CUDA-graph training steps do not support patch_drop_rate > 0 "
+                               "(the kept patches are keyed from the host)")
         if model.training and cfg.mixing:
             raise RuntimeError("CUDA-graph training steps do not support mixup / cutmix > 0 "
                                "(lam and the box come from the host)")
