@@ -109,6 +109,15 @@ def build_arg_parser() -> argparse.ArgumentParser:
                         help="patch dropout (timm PatchDropout; Liu et al. 2022, FLIP): in training every image keeps "
                              "a random max(1, int(N * (1 - rate))) of its N patch tokens (the class / register tokens "
                              "always), so every block runs on fewer tokens; evaluation keeps all; 0 = off")
+    # ---- model EMA (timm ModelEmaV2; DeiT --model-ema) ----
+    parser.add_argument("--model_ema", action="store_true",
+                        help="keep an exponential moving average of the weights (timm ModelEmaV2, DeiT --model-ema), "
+                             "sharded like the master and updated by every optimizer step; it starts as a copy of the "
+                             "initial (or --init_from_full_ckpt) weights, is evaluated after the model at every test "
+                             "epoch and is saved as model_ema in the checkpoints; 4 bytes per sharded parameter")
+    parser.add_argument("--model_ema_decay", type=_ema_decay, default=0.9998,
+                        help="EMA decay d: ema = d * ema + (1 - d) * w after every step (timm train.py 0.9998, DeiT "
+                             "0.99996); in [0, 1), 0 = the EMA is the weights")
     return parser
 
 
@@ -141,6 +150,13 @@ def _patch_drop_rate(s: str) -> float:
     v = float(s)
     if not 0.0 <= v < 1.0:
         raise argparse.ArgumentTypeError(f"--patch_drop_rate must be in [0, 1), got {s}")
+    return v
+
+
+def _ema_decay(s: str) -> float:
+    v = float(s)
+    if not 0.0 <= v < 1.0:
+        raise argparse.ArgumentTypeError(f"--model_ema_decay must be in [0, 1), got {s}")
     return v
 
 

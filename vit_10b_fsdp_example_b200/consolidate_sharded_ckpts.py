@@ -8,7 +8,9 @@ checkpoint layout exists to serve (utils.py:27-28):
 
 reads ``{prefix}_rank_{0..W-1}.ckpt``, concatenates every group's shards, strips the padding, reshapes to the
 parameter shapes (un-flattening flat parameters) and writes a timm-style state_dict
-(``pos_embed`` [1,N,D], ``patch_embed.proj.weight`` [D,3,P,P], ``blocks.{i}.attn.qkv.weight`` ...).
+(``pos_embed`` [1,N,D], ``patch_embed.proj.weight`` [D,3,P,P], ``blocks.{i}.attn.qkv.weight`` ...).  When the
+shards carry a model EMA (``--model_ema``) it is consolidated the same way and written as ``model_ema`` next to
+``model`` (the key DeiT uses).
 """
 from __future__ import annotations
 
@@ -21,7 +23,8 @@ import torch
 from .parallel.layout import UnitLayout
 
 
-def consolidate(ckpts: List[dict]) -> Dict[str, torch.Tensor]:
+def consolidate(ckpts: List[dict], key: str = "model") -> Dict[str, torch.Tensor]:
+    """The full state_dict of the rank files' ``key`` entry: ``model``, or ``model_ema`` for the EMA."""
     md0 = ckpts[0]["shard_metadata"]
     assert md0 is not None, "checkpoint was not written by an FSDP model (shard_metadata is None)"
     world = md0["world_size"]
@@ -35,7 +38,7 @@ def consolidate(ckpts: List[dict]) -> Dict[str, torch.Tensor]:
         lay = UnitLayout.from_metadata(umd)
         full = torch.zeros(lay.full_numel, dtype=torch.float32)
         for r in range(world):
-            sd = by_rank[r]["model"]
+            sd = by_rank[r][key]
             for g in lay.groups:
                 piece = sd[f"{lay.name}.{g.name}"]
                 off = g.full_offset + r * g.shard_len
@@ -61,8 +64,11 @@ def consolidate_files(ckpt_prefix: str, ckpt_suffix: str = "_rank_*.ckpt", save_
     ckpts = [torch.load(p, map_location="cpu", weights_only=False, mmap=True) for p in paths]
     full = consolidate(ckpts)
     if save_path:
+        out = {"model": full, "shard_metadata": None}
+        if all("model_ema" in c for c in ckpts):
+            out["model_ema"] = consolidate(ckpts, key="model_ema")
         os.makedirs(os.path.dirname(os.path.abspath(save_path)), exist_ok=True)
-        torch.save({"model": full, "shard_metadata": None}, save_path)
+        torch.save(out, save_path)
         print(f"consolidated {len(paths)} shard files ({sum(t.numel() for t in full.values()):,} parameters) -> {save_path}")
     return full
 

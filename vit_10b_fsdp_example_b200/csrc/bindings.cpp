@@ -408,23 +408,42 @@ void sumsq(Tensor x, Tensor out) {
 }
 
 void adamw_split(Tensor hi, Tensor lo, Tensor m, Tensor v, Tensor grad, OptT clip_coef, double lr, double beta1,
-                 double beta2, double eps, double wd, int64_t step, OptT hyper) {
+                 double beta2, double eps, double wd, int64_t step, OptT hyper, OptT ema_hi, OptT ema_lo,
+                 double ema_decay) {
     c10::cuda::CUDAGuard guard(hi.device());
     TORCH_CHECK(hi.scalar_type() == at::kBFloat16 && lo.scalar_type() == at::kShort, "hi: bf16, lo: int16");
+    TORCH_CHECK(ema_hi.has_value() == ema_lo.has_value(), "adamw_split: pass both ema_hi and ema_lo, or neither");
+    if (ema_hi.has_value()) {
+        TORCH_CHECK(ema_hi->scalar_type() == at::kBFloat16 && ema_lo->scalar_type() == at::kShort,
+                    "adamw_split: ema_hi must be bf16 and ema_lo int16");
+        TORCH_CHECK(ema_hi->numel() == hi.numel() && ema_lo->numel() == hi.numel(),
+                    "adamw_split: the EMA must have as many elements as the master");
+        TORCH_CHECK(ema_hi->is_contiguous() && ema_lo->is_contiguous() && ema_hi->device() == hi.device() &&
+                        ema_lo->device() == hi.device(), "adamw_split: the EMA must be contiguous, on the master's device");
+        TORCH_CHECK(ema_decay >= 0.0 && ema_decay < 1.0, "adamw_split: ema_decay must be in [0, 1)");
+    }
     const bool gbf = grad.scalar_type() == at::kBFloat16;
     b200::adamw_split(reinterpret_cast<uint16_t*>(hi.data_ptr()), reinterpret_cast<int16_t*>(lo.data_ptr()),
                       f32_ptr(m), f32_ptr(v), grad.data_ptr(), gbf, hi.numel(),
                       clip_coef.has_value() ? f32_ptr(*clip_coef) : nullptr, (float)lr, (float)beta1, (float)beta2,
-                      (float)eps, (float)wd, (int)step, cur_stream(), hyper.has_value() ? f32_ptr(*hyper) : nullptr);
+                      (float)eps, (float)wd, (int)step, cur_stream(), hyper.has_value() ? f32_ptr(*hyper) : nullptr,
+                      ema_hi.has_value() ? reinterpret_cast<uint16_t*>(ema_hi->data_ptr()) : nullptr,
+                      ema_lo.has_value() ? reinterpret_cast<int16_t*>(ema_lo->data_ptr()) : nullptr, (float)ema_decay);
 }
 
 void adamw_fp32(Tensor w, Tensor m, Tensor v, Tensor grad, OptT clip_coef, double lr, double beta1, double beta2,
-                double eps, double wd, int64_t step) {
+                double eps, double wd, int64_t step, OptT ema, double ema_decay) {
     c10::cuda::CUDAGuard guard(w.device());
+    if (ema.has_value()) {
+        TORCH_CHECK(ema->scalar_type() == at::kFloat && ema->numel() == w.numel() && ema->is_contiguous() &&
+                        ema->device() == w.device(), "adamw_fp32: the EMA must be a contiguous fp32 tensor like w");
+        TORCH_CHECK(ema_decay >= 0.0 && ema_decay < 1.0, "adamw_fp32: ema_decay must be in [0, 1)");
+    }
     const bool gbf = grad.scalar_type() == at::kBFloat16;
     b200::adamw_fp32(f32_ptr(w), f32_ptr(m), f32_ptr(v), grad.data_ptr(), gbf, w.numel(),
                      clip_coef.has_value() ? f32_ptr(*clip_coef) : nullptr, (float)lr, (float)beta1, (float)beta2,
-                     (float)eps, (float)wd, (int)step, cur_stream());
+                     (float)eps, (float)wd, (int)step, cur_stream(), ema.has_value() ? f32_ptr(*ema) : nullptr,
+                     (float)ema_decay);
 }
 
 void split_fp32(Tensor w, Tensor hi, Tensor lo) {
@@ -580,8 +599,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("patch_drop_bwd", &patch_drop_bwd);
     m.def("colsum", &colsum);
     m.def("sumsq", &sumsq);
-    m.def("adamw_split", &adamw_split);
-    m.def("adamw_fp32", &adamw_fp32);
+    m.def("adamw_split", &adamw_split, py::arg("hi"), py::arg("lo"), py::arg("m"), py::arg("v"), py::arg("grad"),
+          py::arg("clip_coef"), py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"),
+          py::arg("step"), py::arg("hyper") = py::none(), py::arg("ema_hi") = py::none(),
+          py::arg("ema_lo") = py::none(), py::arg("ema_decay") = 0.0);
+    m.def("adamw_fp32", &adamw_fp32, py::arg("w"), py::arg("m"), py::arg("v"), py::arg("grad"), py::arg("clip_coef"),
+          py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"), py::arg("step"),
+          py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0);
     m.def("split_fp32", &split_fp32);
     m.def("merge_fp32", &merge_fp32);
     m.def("clip_coef", &clip_coef);

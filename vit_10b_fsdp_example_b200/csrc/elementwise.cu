@@ -1066,14 +1066,31 @@ __device__ __forceinline__ void load_grad4(const __nv_bfloat16* g, int64_t i, fl
     out[0] = bf16_lo(v.x), out[1] = bf16_hi(v.x), out[2] = bf16_lo(v.y), out[3] = bf16_hi(v.y);
 }
 
+// Split-fp32 helpers shared by the AdamW update and its EMA: (hi << 16) + lo are the fp32 bits, hi rounded half-up.
+__device__ __forceinline__ float merge_split(uint32_t h, uint32_t l) {
+    return __int_as_float(static_cast<int32_t>(h << 16) + static_cast<int32_t>(static_cast<int16_t>(l)));
+}
+__device__ __forceinline__ void split_bits(float w, uint32_t& h_out, uint32_t& l_out) {
+    const int32_t nb = __float_as_int(w);
+    const int32_t rounded = nb + 0x8000;  // round-half-up: keeps lo in [-32768, 32767] (see split_fp32)
+    const int32_t h = rounded >> 16;
+    h_out = static_cast<uint32_t>(h) & 0xFFFFu;
+    l_out = static_cast<uint32_t>(nb - (h << 16)) & 0xFFFFu;
+}
+
 // 4 elements per thread: 8 B (hi) + 8 B (lo) + 16 B (m) + 16 B (v) + 8/16 B (grad) vector accesses.
-template <typename GradT>
-__global__ void __launch_bounds__(256) adamw_split_kernel(uint16_t* __restrict__ hi, int16_t* __restrict__ lo,
-                                                          float* __restrict__ m, float* __restrict__ v,
-                                                          const GradT* __restrict__ grad, int64_t n,
-                                                          const float* __restrict__ clip_coef, float lr, float beta1,
-                                                          float beta2, float eps, float wd, float bc1, float bc2,
-                                                          const float* __restrict__ hyper) {
+// EMA (model EMA, timm ModelEmaV2): the moving average of the weights is kept in the master's own split form,
+// ema_hi (bf16) + ema_lo (int16), and updated from the new fp32 w while it is still in registers:
+//   ema = fmaf(d, ema, (1 - d) * w)        (1 - d formed in fp32, so d = 0 gives ema == w bitwise)
+// 8 more bytes per element (ema_hi + ema_lo, read and written); hi / lo / m / v are computed exactly as without it.
+template <typename GradT, bool EMA>
+__device__ __forceinline__ void adamw_split_body(uint16_t* __restrict__ hi, int16_t* __restrict__ lo,
+                                                 float* __restrict__ m, float* __restrict__ v,
+                                                 const GradT* __restrict__ grad, int64_t n,
+                                                 const float* __restrict__ clip_coef, float lr, float beta1, float beta2,
+                                                 float eps, float wd, float bc1, float bc2,
+                                                 const float* __restrict__ hyper, uint16_t* __restrict__ ema_hi,
+                                                 int16_t* __restrict__ ema_lo, float ema_decay) {
     const float coef = clip_coef != nullptr ? *clip_coef : 1.0f;
     if (hyper != nullptr) {  // lr and step live on the device so the launch can sit inside a CUDA graph
         lr = hyper[0];
@@ -1084,6 +1101,7 @@ __global__ void __launch_bounds__(256) adamw_split_kernel(uint16_t* __restrict__
         bc2 = -expm1f(hyper[1] * log1pf(beta2 - 1.f));
     }
     const float inv_bc1 = 1.f / bc1, inv_bc2 = 1.f / bc2, decay = 1.f - lr * wd;
+    const float ema_keep = 1.f - ema_decay;
     const int64_t n4 = n / 4;
     for (int64_t q = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; q < n4;
          q += static_cast<int64_t>(gridDim.x) * blockDim.x) {
@@ -1094,10 +1112,15 @@ __global__ void __launch_bounds__(256) adamw_split_kernel(uint16_t* __restrict__
         float4 vv = *reinterpret_cast<const float4*>(v + i);
         float g[4];
         load_grad4(grad, i, g);
+        uint2 ehv, elv;
+        if constexpr (EMA) {
+            ehv = *reinterpret_cast<const uint2*>(ema_hi + i);
+            elv = *reinterpret_cast<const uint2*>(ema_lo + i);
+        }
         const uint32_t hw[4] = {hv.x & 0xFFFFu, hv.x >> 16, hv.y & 0xFFFFu, hv.y >> 16};
         const uint32_t lw[4] = {lv.x & 0xFFFFu, lv.x >> 16, lv.y & 0xFFFFu, lv.y >> 16};
         float mm[4] = {mv.x, mv.y, mv.z, mv.w}, vq[4] = {vv.x, vv.y, vv.z, vv.w};
-        uint32_t ho[4], lo_o[4];
+        uint32_t ho[4], lo_o[4], eho[4], elo[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             const int32_t bits = static_cast<int32_t>(hw[k] << 16) + static_cast<int32_t>(static_cast<int16_t>(lw[k]));
@@ -1111,11 +1134,21 @@ __global__ void __launch_bounds__(256) adamw_split_kernel(uint16_t* __restrict__
             const int32_t h = rounded >> 16;
             ho[k] = static_cast<uint32_t>(h) & 0xFFFFu;
             lo_o[k] = static_cast<uint32_t>(nb - (h << 16)) & 0xFFFFu;
+            if constexpr (EMA) {
+                const uint32_t sh = k & 1 ? 16 : 0;
+                const float e = merge_split(((k < 2 ? ehv.x : ehv.y) >> sh) & 0xFFFFu,
+                                            ((k < 2 ? elv.x : elv.y) >> sh) & 0xFFFFu);
+                split_bits(fmaf(ema_decay, e, ema_keep * w), eho[k], elo[k]);
+            }
         }
         *reinterpret_cast<uint2*>(hi + i) = make_uint2(ho[0] | (ho[1] << 16), ho[2] | (ho[3] << 16));
         *reinterpret_cast<uint2*>(lo + i) = make_uint2(lo_o[0] | (lo_o[1] << 16), lo_o[2] | (lo_o[3] << 16));
         *reinterpret_cast<float4*>(m + i) = make_float4(mm[0], mm[1], mm[2], mm[3]);
         *reinterpret_cast<float4*>(v + i) = make_float4(vq[0], vq[1], vq[2], vq[3]);
+        if constexpr (EMA) {
+            *reinterpret_cast<uint2*>(ema_hi + i) = make_uint2(eho[0] | (eho[1] << 16), eho[2] | (eho[3] << 16));
+            *reinterpret_cast<uint2*>(ema_lo + i) = make_uint2(elo[0] | (elo[1] << 16), elo[2] | (elo[3] << 16));
+        }
     }
     // scalar tail (n not a multiple of 4)
     for (int64_t i = n4 * 4 + static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
@@ -1133,16 +1166,47 @@ __global__ void __launch_bounds__(256) adamw_split_kernel(uint16_t* __restrict__
         const int32_t h = rounded >> 16;
         hi[i] = static_cast<uint16_t>(h & 0xFFFF);
         lo[i] = static_cast<int16_t>(nb - (h << 16));
+        if constexpr (EMA) {
+            const float e = merge_split(ema_hi[i], static_cast<uint16_t>(ema_lo[i]));
+            uint32_t eh, el;
+            split_bits(fmaf(ema_decay, e, ema_keep * w), eh, el);
+            ema_hi[i] = static_cast<uint16_t>(eh);
+            ema_lo[i] = static_cast<int16_t>(static_cast<uint16_t>(el));
+        }
     }
 }
 
-// Plain fp32-master variant (used when the compute dtype is fp32).
 template <typename GradT>
-__global__ void __launch_bounds__(256) adamw_fp32_kernel(float* __restrict__ w, float* __restrict__ m,
-                                                         float* __restrict__ v, const GradT* __restrict__ grad,
-                                                         int64_t n, const float* __restrict__ clip_coef, float lr,
-                                                         float beta1, float beta2, float eps, float wd, float bc1,
-                                                         float bc2) {
+__global__ void __launch_bounds__(256) adamw_split_kernel(uint16_t* __restrict__ hi, int16_t* __restrict__ lo,
+                                                          float* __restrict__ m, float* __restrict__ v,
+                                                          const GradT* __restrict__ grad, int64_t n,
+                                                          const float* __restrict__ clip_coef, float lr, float beta1,
+                                                          float beta2, float eps, float wd, float bc1, float bc2,
+                                                          const float* __restrict__ hyper) {
+    adamw_split_body<GradT, false>(hi, lo, m, v, grad, n, clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2, hyper,
+                                   nullptr, nullptr, 0.f);
+}
+
+template <typename GradT>
+__global__ void __launch_bounds__(256) adamw_split_ema_kernel(uint16_t* __restrict__ hi, int16_t* __restrict__ lo,
+                                                              float* __restrict__ m, float* __restrict__ v,
+                                                              const GradT* __restrict__ grad, int64_t n,
+                                                              const float* __restrict__ clip_coef, float lr,
+                                                              float beta1, float beta2, float eps, float wd, float bc1,
+                                                              float bc2, const float* __restrict__ hyper,
+                                                              uint16_t* __restrict__ ema_hi,
+                                                              int16_t* __restrict__ ema_lo, float ema_decay) {
+    adamw_split_body<GradT, true>(hi, lo, m, v, grad, n, clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2, hyper,
+                                  ema_hi, ema_lo, ema_decay);
+}
+
+// Plain fp32-master variant (used when the compute dtype is fp32); the EMA is a plain fp32 shard here.
+template <typename GradT, bool EMA>
+__device__ __forceinline__ void adamw_fp32_body(float* __restrict__ w, float* __restrict__ m, float* __restrict__ v,
+                                                const GradT* __restrict__ grad, int64_t n,
+                                                const float* __restrict__ clip_coef, float lr, float beta1, float beta2,
+                                                float eps, float wd, float bc1, float bc2, float* __restrict__ ema,
+                                                float ema_decay) {
     const float coef = clip_coef != nullptr ? *clip_coef : 1.0f;
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
          i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
@@ -1151,8 +1215,28 @@ __global__ void __launch_bounds__(256) adamw_fp32_kernel(float* __restrict__ w, 
         const float vi = beta2 * v[i] + (1.f - beta2) * g * g;
         m[i] = mi;
         v[i] = vi;
-        w[i] = w[i] * (1.f - lr * wd) - lr * (mi / bc1) / (sqrtf(vi / bc2) + eps);
+        const float wi = w[i] * (1.f - lr * wd) - lr * (mi / bc1) / (sqrtf(vi / bc2) + eps);
+        w[i] = wi;
+        if constexpr (EMA) ema[i] = fmaf(ema_decay, ema[i], (1.f - ema_decay) * wi);
     }
+}
+
+template <typename GradT>
+__global__ void __launch_bounds__(256) adamw_fp32_kernel(float* __restrict__ w, float* __restrict__ m,
+                                                         float* __restrict__ v, const GradT* __restrict__ grad,
+                                                         int64_t n, const float* __restrict__ clip_coef, float lr,
+                                                         float beta1, float beta2, float eps, float wd, float bc1,
+                                                         float bc2) {
+    adamw_fp32_body<GradT, false>(w, m, v, grad, n, clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2, nullptr, 0.f);
+}
+
+template <typename GradT>
+__global__ void __launch_bounds__(256) adamw_fp32_ema_kernel(float* __restrict__ w, float* __restrict__ m,
+                                                             float* __restrict__ v, const GradT* __restrict__ grad,
+                                                             int64_t n, const float* __restrict__ clip_coef, float lr,
+                                                             float beta1, float beta2, float eps, float wd, float bc1,
+                                                             float bc2, float* __restrict__ ema, float ema_decay) {
+    adamw_fp32_body<GradT, true>(w, m, v, grad, n, clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2, ema, ema_decay);
 }
 
 // Split an fp32 tensor into (hi bf16, lo int16) and back.
@@ -1493,35 +1577,57 @@ void sumsq(const void* x, bool is_bf16, int64_t n, float* out, cudaStream_t stre
 
 void adamw_split(uint16_t* hi, int16_t* lo, float* m, float* v, const void* grad, bool grad_is_bf16, int64_t n,
                  const float* clip_coef, float lr, float beta1, float beta2, float eps, float wd, int step,
-                 cudaStream_t stream, const float* hyper) {
+                 cudaStream_t stream, const float* hyper, uint16_t* ema_hi, int16_t* ema_lo, float ema_decay) {
+    if ((ema_hi == nullptr) != (ema_lo == nullptr))
+        throw std::runtime_error("adamw_split: the EMA needs both ema_hi and ema_lo (or neither)");
     const int grid = static_cast<int>(std::min<int64_t>((n / 4 + 255) / 256 + 1, sm_count() * 16));
     if (grid == 0) return;
     // 1 - beta^t in double: in fp32, 1 - powf(0.999f, 2) keeps only the rounding error of powf (1.5e-5 of 0.002)
     const float bc1 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta1), static_cast<double>(step)));
     const float bc2 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta2), static_cast<double>(step)));
-    if (grad_is_bf16)
+    if (ema_hi != nullptr) {
+        if (grad_is_bf16)
+            adamw_split_ema_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
+                hi, lo, m, v, static_cast<const __nv_bfloat16*>(grad), n, clip_coef, lr, beta1, beta2, eps, wd, bc1,
+                bc2, hyper, ema_hi, ema_lo, ema_decay);
+        else
+            adamw_split_ema_kernel<float><<<grid, 256, 0, stream>>>(hi, lo, m, v, static_cast<const float*>(grad), n,
+                                                                   clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2,
+                                                                   hyper, ema_hi, ema_lo, ema_decay);
+    } else if (grad_is_bf16) {
         adamw_split_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(hi, lo, m, v, static_cast<const __nv_bfloat16*>(grad),
                                                                    n, clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2,
                                                                    hyper);
-    else
+    } else {
         adamw_split_kernel<float><<<grid, 256, 0, stream>>>(hi, lo, m, v, static_cast<const float*>(grad), n, clip_coef,
                                                            lr, beta1, beta2, eps, wd, bc1, bc2, hyper);
+    }
     check_launch("adamw_split");
 }
 
 void adamw_fp32(float* w, float* m, float* v, const void* grad, bool grad_is_bf16, int64_t n, const float* clip_coef,
-                float lr, float beta1, float beta2, float eps, float wd, int step, cudaStream_t stream) {
+                float lr, float beta1, float beta2, float eps, float wd, int step, cudaStream_t stream, float* ema,
+                float ema_decay) {
     const int grid = static_cast<int>(std::min<int64_t>((n + 255) / 256, sm_count() * 16));
     if (grid == 0) return;
     // 1 - beta^t in double: in fp32, 1 - powf(0.999f, 2) keeps only the rounding error of powf (1.5e-5 of 0.002)
     const float bc1 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta1), static_cast<double>(step)));
     const float bc2 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta2), static_cast<double>(step)));
-    if (grad_is_bf16)
+    if (ema != nullptr) {
+        if (grad_is_bf16)
+            adamw_fp32_ema_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
+                w, m, v, static_cast<const __nv_bfloat16*>(grad), n, clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2, ema,
+                ema_decay);
+        else
+            adamw_fp32_ema_kernel<float><<<grid, 256, 0, stream>>>(w, m, v, static_cast<const float*>(grad), n, clip_coef,
+                                                                  lr, beta1, beta2, eps, wd, bc1, bc2, ema, ema_decay);
+    } else if (grad_is_bf16) {
         adamw_fp32_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(w, m, v, static_cast<const __nv_bfloat16*>(grad), n,
                                                                   clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2);
-    else
+    } else {
         adamw_fp32_kernel<float><<<grid, 256, 0, stream>>>(w, m, v, static_cast<const float*>(grad), n, clip_coef, lr,
                                                           beta1, beta2, eps, wd, bc1, bc2);
+    }
     check_launch("adamw_fp32");
 }
 

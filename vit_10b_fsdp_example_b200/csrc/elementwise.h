@@ -75,11 +75,16 @@ void qk_norm_bwd(__nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* qkv, in
 void sumsq(const void* x, bool is_bf16, int64_t n, float* out, cudaStream_t stream);
 
 // hyper (optional, device): [lr, step] override the host values (CUDA-graph friendly)
+// ema_hi / ema_lo (optional, both or neither): the model EMA in split form, updated in the same pass as
+// ema = fmaf(ema_decay, ema, (1 - ema_decay) * w) from the new master w; null = no EMA (the plain kernel)
 void adamw_split(uint16_t* hi, int16_t* lo, float* m, float* v, const void* grad, bool grad_is_bf16, int64_t n,
                  const float* clip_coef, float lr, float beta1, float beta2, float eps, float wd, int step,
-                 cudaStream_t stream, const float* hyper = nullptr);
+                 cudaStream_t stream, const float* hyper = nullptr, uint16_t* ema_hi = nullptr,
+                 int16_t* ema_lo = nullptr, float ema_decay = 0.f);
+// ema (optional): fp32 model EMA, same recurrence
 void adamw_fp32(float* w, float* m, float* v, const void* grad, bool grad_is_bf16, int64_t n, const float* clip_coef,
-                float lr, float beta1, float beta2, float eps, float wd, int step, cudaStream_t stream);
+                float lr, float beta1, float beta2, float eps, float wd, int step, cudaStream_t stream,
+                float* ema = nullptr, float ema_decay = 0.f);
 void split_fp32(const float* w, uint16_t* hi, int16_t* lo, int64_t n, cudaStream_t stream);
 void merge_fp32(const uint16_t* hi, const int16_t* lo, float* w, int64_t n, cudaStream_t stream);
 void clip_coef(const float* sumsq_in, float max_norm, float* coef, float* norm_out, cudaStream_t stream);

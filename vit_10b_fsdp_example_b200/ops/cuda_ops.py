@@ -631,13 +631,24 @@ def clip_coef(sumsq_t, max_norm: float):
     return coef, norm
 
 
-def adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int):
-    _C.adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step)
+def adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, ema=None, ema_decay: float = 0.0):
+    """ema: optional fp32 model EMA, updated in the same pass as ema = fmaf(d, ema, (1 - d) * w_new)."""
+    if ema is None:
+        _C.adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step)
+    else:
+        _C.adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, ema, float(ema_decay))
 
 
-def adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, hyper=None):
-    """hyper: optional device tensor [lr, step] that overrides the host scalars (CUDA-graph replay)."""
-    _C.adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, hyper)
+def adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, hyper=None, ema=None,
+                ema_decay: float = 0.0):
+    """hyper: optional device tensor [lr, step] that overrides the host scalars (CUDA-graph replay).
+    ema: optional (ema_hi, ema_lo), the model EMA in the master's split form, updated in the same pass as
+    ema = fmaf(d, ema, (1 - d) * w_new) with d = ema_decay."""
+    if ema is None:
+        _C.adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, hyper)
+    else:
+        _C.adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, hyper, ema[0], ema[1],
+                       float(ema_decay))
 
 
 def split_fp32(w, hi, lo):

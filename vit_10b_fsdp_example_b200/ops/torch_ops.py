@@ -538,7 +538,23 @@ def clip_coef(sumsq_t, max_norm: float):
     return torch.clamp(max_norm / (norm + 1e-6), max=1.0), norm
 
 
-def adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int):
+def ema_update(ema, w, decay: float):
+    """Model EMA step as the device computes it: ema = fmaf(d, ema, (1 - d) * w) in fp32, with d and 1 - d rounded to
+    fp32.  The fused multiply-add is emulated in fp64, where the product of two fp32 values is exact; the sum is then
+    rounded to fp64 and to fp32, which is one rounding more than fmaf (it can differ in the last bit on a tie)."""
+    d = float(np.float32(decay))
+    keep = torch.mul(w, float(np.float32(1.0) - np.float32(decay)))  # fp32 product, as on the device
+    ema.copy_((ema.double() * d + keep.double()).float())
+
+
+def adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, ema=None, ema_decay: float = 0.0):
+    """ema: optional fp32 model EMA, updated from the new w (see ema_update)."""
+    _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step)
+    if ema is not None:
+        ema_update(ema, w, ema_decay)
+
+
+def _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int):
     g = _f32(grad)
     if clip is not None:
         g = g * clip
@@ -566,8 +582,15 @@ def merge_fp32(hi, lo, w):
     w.copy_(bits.view(torch.float32))
 
 
-def adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, hyper=None):
+def adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, hyper=None, ema=None,
+                ema_decay: float = 0.0):
+    """ema: optional (ema_hi, ema_lo), the model EMA in split form."""
     w = torch.empty(hi.shape, dtype=torch.float32, device=hi.device)
     merge_fp32(hi, lo, w)
-    adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step)
+    _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step)
     split_fp32(w, hi, lo)
+    if ema is not None:
+        e = torch.empty(hi.shape, dtype=torch.float32, device=hi.device)
+        merge_fp32(ema[0], ema[1], e)
+        ema_update(e, w, ema_decay)
+        split_fp32(e, ema[0], ema[1])

@@ -69,6 +69,10 @@ class FsdpUnit:
         self.exp_avg: Optional[torch.Tensor] = None
         self.exp_avg_sq: Optional[torch.Tensor] = None
         self.shard_grad: Optional[torch.Tensor] = None
+        self.ema_hi: Optional[torch.Tensor] = None   # model EMA, split like the master (bf16 compute mode)
+        self.ema_lo: Optional[torch.Tensor] = None
+        self.ema: Optional[torch.Tensor] = None      # model EMA, fp32 (fp32 compute mode)
+        self.use_ema = False                         # inside FSDPViT.ema_weights(): compute from the EMA
         self.full: Optional[torch.Tensor] = None     # gathered parameters (compute dtype) while resident
         self.full_grad: Optional[torch.Tensor] = None
         self.gather_event = None
@@ -77,6 +81,8 @@ class FsdpUnit:
 
     @property
     def compute_shard(self) -> torch.Tensor:
+        if self.use_ema:
+            return self.ema_hi if self.ema_hi is not None else self.ema
         return self.hi if self.hi is not None else self.master
 
 
@@ -87,7 +93,7 @@ class FSDPViT:
                  reshard_after_forward: bool = True, flatten_parameters: bool = False, grad_ckpt: bool = True,
                  run_without_fsdp: bool = False, shard_on_cpu: bool = False, backend: str = "torchdist",
                  seed: int = 0, init_device: str = "cpu", verbose_build=None, fuse_all_gather: bool = True,
-                 ckpt_keep_blocks: int = 0):
+                 ckpt_keep_blocks: int = 0, model_ema: bool = False):
         self.cfg = vcfg
         self.device = torch.device(device) if device is not None else torch.device("cpu")
         self.dtype = dtype
@@ -163,6 +169,11 @@ class FSDPViT:
         self._init_unit(self.root, lambda g, d: vit.init_root_params(vcfg, g, d), seed * 100003, gen_device)
         self.blocks = self.units
         self.all_units = self.units + [self.root]
+        # model EMA: a sharded moving average of the weights, kept like the master and updated by the AdamW kernel
+        self.has_ema = bool(model_ema)
+        if self.has_ema:
+            self._alloc_ema()
+            self.reset_ema()
 
         # ---- transient buffers ----
         self._setup_buffers()
@@ -203,6 +214,72 @@ class FSDPViT:
             if unit.master is None:
                 unit.master = self.backend.alloc_shard(n, torch.float32)
             unit.master.copy_(shard_fp32)
+
+    def _alloc_ema(self) -> None:
+        """One EMA shard per unit, in unit order on every rank (at W > 1 under sm100 ``ema_hi`` is symmetric memory, so
+        the EMA evaluation can all-gather from it and the AG-fused GEMMs can pull it; the allocation is collective)."""
+        for u in self.all_units:
+            n = u.layout.shard_numel
+            if self.split_master:
+                u.ema_hi = self.backend.alloc_shard(n, torch.bfloat16)
+                u.ema_lo = torch.zeros(n, dtype=torch.int16, device=self.device)
+            else:
+                u.ema = self.backend.alloc_shard(n, torch.float32)
+
+    def reset_ema(self) -> None:
+        """Start the EMA from the current weights (a bitwise copy of the master)."""
+        for u in self.all_units:
+            if self.split_master:
+                u.ema_hi.copy_(u.hi)
+                u.ema_lo.copy_(u.lo)
+            else:
+                u.ema.copy_(u.master)
+        self.backend.params_updated()
+
+    def ema_operand(self, unit: FsdpUnit):
+        """What the AdamW launch of `unit` takes as its EMA: (ema_hi, ema_lo), the fp32 EMA, or None."""
+        if not self.has_ema:
+            return None
+        return (unit.ema_hi, unit.ema_lo) if self.split_master else unit.ema
+
+    def ema_fp32(self, unit: FsdpUnit) -> torch.Tensor:
+        """This rank's fp32 EMA shard (reconstructed exactly from the split representation)."""
+        if not self.split_master:
+            return unit.ema
+        out = torch.empty(unit.layout.shard_numel, dtype=torch.float32, device=self.device)
+        self.ops.merge_fp32(unit.ema_hi, unit.ema_lo, out)
+        return out
+
+    def _install_ema(self, unit: FsdpUnit, shard_fp32: torch.Tensor) -> None:
+        if self.split_master:
+            self.ops.split_fp32(shard_fp32, unit.ema_hi, unit.ema_lo)
+        else:
+            unit.ema.copy_(shard_fp32)
+
+    @contextlib.contextmanager
+    def ema_weights(self):
+        """``with model.ema_weights(): logits = model(images)``: every unit computes from its EMA shard instead of the
+        master.  The all-gather source, the AG-fused GEMM specs and (W = 1) the aliased ``u.full`` all follow
+        ``compute_shard``; the EMA's bf16 compute weights are exactly its ``hi`` half, so nothing is converted or
+        copied.  Only host-side pointers change: a captured CUDA graph keeps the tensors it recorded."""
+        if not self.has_ema:
+            raise RuntimeError("this model has no EMA (construct it with model_ema=True, CLI --model_ema)")
+        if any(u.use_ema for u in self.all_units):
+            raise RuntimeError("ema_weights() is already active")
+
+        def swap(on: bool) -> None:
+            for u in self.all_units:
+                u.use_ema = on
+                u.gather_event = None  # a gather of the other weights is stale (as after _begin_step)
+                u.fused_pending = ()
+                if self._alias:
+                    u.full = u.compute_shard
+
+        swap(True)
+        try:
+            yield self
+        finally:
+            swap(False)
 
     def master_fp32(self, unit: FsdpUnit) -> torch.Tensor:
         """This rank's fp32 master shard (reconstructed exactly from the split representation)."""
@@ -646,22 +723,50 @@ class FSDPViT:
                 out[f"{u.name}.{g.name}"] = m[g.shard_offset: g.shard_offset + g.shard_len].clone()
         return out
 
+    def ema_state_dict(self) -> Dict[str, torch.Tensor]:
+        """This rank's EMA shards, in the layout of ``state_dict`` (checkpoint key ``model_ema``)."""
+        if not self.has_ema:
+            raise RuntimeError("this model has no EMA")
+        out = {}
+        for u in self.all_units:
+            e = self.ema_fp32(u).detach().cpu()
+            for g in u.layout.groups:
+                out[f"{u.name}.{g.name}"] = e[g.shard_offset: g.shard_offset + g.shard_len].clone()
+        return out
+
+    def _shards_from_state(self, state: Dict[str, torch.Tensor], u: FsdpUnit) -> torch.Tensor:
+        m = torch.empty(u.layout.shard_numel, dtype=torch.float32)
+        for g in u.layout.groups:
+            t = state[f"{u.name}.{g.name}"]
+            assert t.numel() == g.shard_len, f"shard size mismatch for {u.name}.{g.name} (world size changed?)"
+            m[g.shard_offset: g.shard_offset + g.shard_len].copy_(t)
+        return m.to(self.device)
+
     def load_state_dict(self, state: Dict[str, torch.Tensor], shard_metadata: Optional[dict] = None) -> None:
+        """Restores the master shards (the EMA, if any, is left alone: see ``load_ema_state_dict``)."""
         if shard_metadata and "step_count" in shard_metadata:
             self.step_count = int(shard_metadata["step_count"])
         for u in self.all_units:
-            m = torch.empty(u.layout.shard_numel, dtype=torch.float32)
-            for g in u.layout.groups:
-                t = state[f"{u.name}.{g.name}"]
-                assert t.numel() == g.shard_len, f"shard size mismatch for {u.name}.{g.name} (world size changed?)"
-                m[g.shard_offset: g.shard_offset + g.shard_len].copy_(t)
-            self._install_master(u, m.to(self.device))
+            self._install_master(u, self._shards_from_state(state, u))
         self.backend.params_updated()
 
-    def load_full_state_dict(self, full: Dict[str, torch.Tensor]) -> None:
+    def load_ema_state_dict(self, state: Dict[str, torch.Tensor]) -> None:
+        """Restores the EMA shards from a rank checkpoint's ``model_ema``."""
+        if not self.has_ema:
+            raise RuntimeError("this model has no EMA")
+        for u in self.all_units:
+            self._install_ema(u, self._shards_from_state(state, u))
+        self.backend.params_updated()
+
+    def load_full_state_dict(self, full: Dict[str, torch.Tensor], ema: bool = False) -> None:
         """Initialise this rank's shards from a *consolidated* (unsharded, timm-style) state_dict, e.g. the output
         of ``consolidate_sharded_ckpts``: the way to continue a run on a different number of GPUs, which per-rank
-        shard files alone cannot do (``load_state_dict`` asserts the world size is unchanged)."""
+        shard files alone cannot do (``load_state_dict`` asserts the world size is unchanged).
+
+        ema=False loads the weights, and a model with an EMA starts its EMA from them; ema=True loads the EMA only
+        (a consolidated checkpoint's ``model_ema``), with the same checks."""
+        if ema and not self.has_ema:
+            raise RuntimeError("this model has no EMA")
         has_qk = any(k.endswith(("attn.q_norm.weight", "attn.k_norm.weight")) for k in full)
         if self.cfg.qk_norm and not has_qk:
             raise ValueError("this model uses --qk_norm, but the checkpoint has no attn.q_norm / attn.k_norm "
@@ -691,7 +796,12 @@ class FSDPViT:
                 buf[p.full_offset: p.full_offset + p.numel].copy_(t.reshape(-1))
             shard = torch.zeros(lay.shard_numel, dtype=torch.float32)
             lay.shard_from_full(buf, self.shard_rank, shard)
-            self._install_master(u, shard.to(self.device))
+            if ema:
+                self._install_ema(u, shard.to(self.device))
+            else:
+                self._install_master(u, shard.to(self.device))
+        if self.has_ema and not ema:
+            self.reset_ema()
         self.backend.params_updated()
 
     def check_mlp_form(self, full: Dict[str, torch.Tensor]) -> None:
@@ -767,4 +877,5 @@ class FSDPViT:
                 f"image={c.image_size}, patch={c.patch_size}, dim={c.embed_dim}, heads={c.num_heads}, "
                 f"blocks={c.num_blocks}, mlp_ratio={c.mlp_ratio}, classes={c.num_classes}, "
                 f"grad_ckpt={self.grad_ckpt}, flatten={self.flatten_parameters}, "
+                f"{'model_ema=True, ' if self.has_ema else ''}"
                 f"params={self.num_parameters():,}, sharded={self.num_sharded_parameters():,})")

@@ -7,26 +7,40 @@ single parameter group: decoupled weight decay is applied to *every* tensor, bia
 
 One fused kernel per unit reads the reduced gradient shard, applies the clip coefficient armed by
 ``model.clip_grad_norm_`` (a device scalar: no host sync, no separate scaling pass), updates m / v and the
-split-fp32 master, and thereby also produces the bf16 shard the next all-gather ships.
+split-fp32 master, and thereby also produces the bf16 shard the next all-gather ships.  With a model EMA
+(``FSDPViT(model_ema=True)``, ``model_ema_decay`` here) the same kernel also updates the EMA from the new master while
+it is in registers: ``ema = d * ema + (1 - d) * w`` (timm ModelEmaV2 with a fixed decay).
 """
 from __future__ import annotations
 
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 
 
 class ShardedAdamW:
     def __init__(self, model, lr: float = 1e-3, weight_decay: float = 1e-2, betas=(0.9, 0.999), eps: float = 1e-8,
-                 fuse_into_reduce_scatter: bool = False):
+                 fuse_into_reduce_scatter: bool = False, model_ema_decay: Optional[float] = None):
         """fuse_into_reduce_scatter: apply the update of each unit inside its gradient reduce-scatter kernel while
         backward is still running (sm100 backend, world > 1).  Only legal when gradient clipping is disabled,
-        because clipping needs the norm of the whole gradient before any parameter changes."""
+        because clipping needs the norm of the whole gradient before any parameter changes.  A model with an EMA
+        never takes this route: the reduce-scatter kernel has no EMA operand, so its units are updated by step().
+
+        model_ema_decay: the EMA decay d in [0, 1); required exactly when the model has an EMA."""
+        has_ema = bool(getattr(model, "has_ema", False))
+        if has_ema and model_ema_decay is None:
+            raise ValueError("the model has an EMA: pass model_ema_decay")
+        if model_ema_decay is not None:
+            if not has_ema:
+                raise ValueError("model_ema_decay needs a model with an EMA (FSDPViT(model_ema=True))")
+            if not 0.0 <= float(model_ema_decay) < 1.0:
+                raise ValueError(f"model_ema_decay must be in [0, 1), got {model_ema_decay}")
+        self.ema_decay = float(model_ema_decay) if has_ema else None
         self.model = model
         self.param_groups = [dict(lr=lr, weight_decay=weight_decay, betas=tuple(betas), eps=eps)]
         self.state: Dict[str, dict] = {u.name: {"step": 0} for u in model.all_units}
         self.fused = bool(fuse_into_reduce_scatter and model.use_fsdp and model.world > 1 and model.split_master
-                          and getattr(model.backend, "supports_fused_adam", False))
+                          and getattr(model.backend, "supports_fused_adam", False) and not has_ema)
         self._done_in_backward = set()
         if self.fused:
             model._fused_opt = self
@@ -66,11 +80,19 @@ class ShardedAdamW:
                 continue  # already updated inside its reduce-scatter kernel
             st = self.state[u.name]
             st["step"] += 1
+            ema = model.ema_operand(u) if self.ema_decay is not None else None
             if model.split_master:
-                ops.adamw_split(u.hi, u.lo, u.exp_avg, u.exp_avg_sq, u.shard_grad, clip, lr, b1, b2, eps, wd, st["step"],
-                                hyper)
-            else:
+                if ema is None:
+                    ops.adamw_split(u.hi, u.lo, u.exp_avg, u.exp_avg_sq, u.shard_grad, clip, lr, b1, b2, eps, wd,
+                                    st["step"], hyper)
+                else:
+                    ops.adamw_split(u.hi, u.lo, u.exp_avg, u.exp_avg_sq, u.shard_grad, clip, lr, b1, b2, eps, wd,
+                                    st["step"], hyper, ema=ema, ema_decay=self.ema_decay)
+            elif ema is None:
                 ops.adamw_fp32(u.master, u.exp_avg, u.exp_avg_sq, u.shard_grad, clip, lr, b1, b2, eps, wd, st["step"])
+            else:
+                ops.adamw_fp32(u.master, u.exp_avg, u.exp_avg_sq, u.shard_grad, clip, lr, b1, b2, eps, wd, st["step"],
+                               ema=ema, ema_decay=self.ema_decay)
         self._done_in_backward.clear()
         model._clip_coef = None
         model.backend.params_updated()
@@ -103,4 +125,5 @@ class ShardedAdamW:
         g = self.param_groups[0]
         return (f"ShardedAdamW(lr={g['lr']}, betas={g['betas']}, eps={g['eps']}, weight_decay={g['weight_decay']}, "
                 f"units={len(self.model.all_units)}, clip_fused_into_update={not self.fused}, "
-                f"fused_into_reduce_scatter={self.fused})")
+                f"fused_into_reduce_scatter={self.fused}"
+                f"{'' if self.ema_decay is None else f', model_ema_decay={self.ema_decay}'})")

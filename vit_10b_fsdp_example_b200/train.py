@@ -78,6 +78,7 @@ def build_fsdp_vit_model(cfg, rt: Runtime) -> FSDPViT:
         backend=resolve_backend(cfg, rt.device), seed=cfg.seed, verbose_build=rt.master_print,
         init_device=resolve_init_device(cfg, rt.device),
         ckpt_keep_blocks=keep if rt.device.type == "cuda" else max(0, keep),
+        model_ema=bool(getattr(cfg, "model_ema", False)),
     )
 
 
@@ -87,7 +88,8 @@ class TrainStep:
     In FSDP mode the gradients leave ``forward_backward`` already reduce-scattered (mean) and the clip coefficient is
     computed from the norm of the full gradient (reference :266-270); in ``--run_without_fsdp`` mode they were
     all-reduced inside ``forward_backward`` (reference :273) and the same clip applies to the replicated gradient.
-    Without clipping the AdamW update is fused into each unit's reduce-scatter kernel (sm100 backend).
+    Without clipping the AdamW update is fused into each unit's reduce-scatter kernel (sm100 backend), except with a
+    model EMA: that is updated by the stand-alone AdamW kernel, so every unit takes that route.
     """
 
     def __init__(self, model: FSDPViT, cfg, device: torch.device):
@@ -95,7 +97,8 @@ class TrainStep:
         self.clip = float(cfg.clip_grad_norm)
         want_graph = bool(getattr(cfg, "cuda_graph", False)) and device.type == "cuda"
         self.optimizer = ShardedAdamW(model, lr=cfg.lr, weight_decay=cfg.weight_decay,
-                                      fuse_into_reduce_scatter=self.clip <= 0 and not want_graph)
+                                      fuse_into_reduce_scatter=self.clip <= 0 and not want_graph and not model.has_ema,
+                                      model_ema_decay=float(cfg.model_ema_decay) if model.has_ema else None)
         self.graph: Optional[GraphedTrainStep] = (
             GraphedTrainStep(model, self.optimizer, self.clip) if want_graph else None)
 
@@ -200,23 +203,34 @@ class Trainer:
 
         if getattr(cfg, "init_from_full_ckpt", ""):
             full = torch.load(cfg.init_from_full_ckpt, map_location="cpu", weights_only=False)
-            state = normalize_full_state_dict_keys(full.get("model", full))
-            mcfg = self.model.cfg
-            self.model.check_prefix_tokens(state)  # before resampling: a wrong prefix layout is named, not resampled
-            if "pos_embed" in state:
-                pos = state["pos_embed"]
-                P = 0 if mcfg.no_embed_class else mcfg.num_prefix_tokens  # rows of pos_embed that are not the grid
-                state["pos_embed"] = resize_pos_embed(pos, mcfg.num_patches, mcfg.embed_dim, num_prefix_tokens=P)
-                if state["pos_embed"] is not pos:
-                    say(f"pos_embed resampled from {pos.shape[1] - P} to {mcfg.num_patches} tokens (bicubic)")
-            self.model.load_full_state_dict(state)
+            self.model.load_full_state_dict(self._full_state(full.get("model", full)))
             say(f"parameters initialised from the consolidated checkpoint {cfg.init_from_full_ckpt}")
+            if self.model.has_ema:
+                if isinstance(full.get("model_ema"), dict):
+                    self.model.load_full_state_dict(self._full_state(full["model_ema"]), ema=True)
+                    say("model EMA initialised from the checkpoint's model_ema")
+                else:
+                    say("the checkpoint has no model_ema: the model EMA starts from the loaded weights")
             del full
         os.makedirs(cfg.ckpt_dir, exist_ok=True)
         if cfg.resume_epoch > 0:  # every rank restores its own shard file
             load_ckpt(self._ckpt_path(cfg.resume_epoch), self.model, self.optimizer, self.lr_scheduler)
         self.loss_meter = SmoothedValue(window_size=5)
         self.time_meter = SmoothedValue(window_size=5)
+
+    def _full_state(self, state: dict) -> dict:
+        """A consolidated state_dict made ready for load_full_state_dict: wrapper prefixes stripped, the prefix-token
+        layout checked, pos_embed resampled to this model's grid."""
+        say, mcfg = self.rt.master_print, self.model.cfg
+        state = normalize_full_state_dict_keys(state)
+        self.model.check_prefix_tokens(state)  # before resampling: a wrong prefix layout is named, not resampled
+        if "pos_embed" in state:
+            pos = state["pos_embed"]
+            P = 0 if mcfg.no_embed_class else mcfg.num_prefix_tokens  # rows of pos_embed that are not the grid
+            state["pos_embed"] = resize_pos_embed(pos, mcfg.num_patches, mcfg.embed_dim, num_prefix_tokens=P)
+            if state["pos_embed"] is not pos:
+                say(f"pos_embed resampled from {pos.shape[1] - P} to {mcfg.num_patches} tokens (bicubic)")
+        return state
 
     def _ckpt_path(self, epoch: int) -> str:
         # One file per *global* rank.  The reference keys the files by the host-local ordinal (:220,247,298), which is
@@ -276,6 +290,10 @@ class Trainer:
             if epoch % cfg.test_epoch_interval == 0 or last:
                 accuracy, _, _ = evaluate(rt, self.val_loader, self.model, max_steps=cfg.max_steps)
                 rt.master_print(f"accuracy on val: {accuracy:.4f}")
+                if self.model.has_ema:
+                    with self.model.ema_weights():
+                        accuracy, _, _ = evaluate(rt, self.val_loader, self.model, max_steps=cfg.max_steps)
+                    rt.master_print(f"accuracy of the EMA on val: {accuracy:.4f}")
         return self.model, self.optimizer, self.lr_scheduler
 
 

@@ -2,8 +2,9 @@
 
 Layout kept compatible with the reference: one ``torch.save`` file per rank per epoch named
 ``epoch_{E}_rank_{R}.ckpt`` holding exactly four keys -- ``model`` (this rank's shards), ``shard_metadata``
-(``None`` when not FSDP), ``optimizer`` and ``lr_scheduler``.  Every rank writes its own file; loading goes
-through the host (``map_location='cpu'``).  ``consolidate_sharded_ckpts`` rebuilds a full state_dict.
+(``None`` when not FSDP), ``optimizer`` and ``lr_scheduler`` -- plus a fifth, ``model_ema`` (this rank's EMA shards,
+same layout as ``model``), only when the model keeps an EMA (``--model_ema``).  Every rank writes its own file; loading
+goes through the host (``map_location='cpu'``).  ``consolidate_sharded_ckpts`` rebuilds a full state_dict.
 """
 from __future__ import annotations
 
@@ -21,6 +22,8 @@ def save_ckpt(ckpt_path: str, model, optimizer, lr_scheduler, master_only: bool 
         "optimizer": optimizer.state_dict(),
         "lr_scheduler": lr_scheduler.state_dict(),
     }
+    if getattr(model, "has_ema", False):
+        ckpt["model_ema"] = model.ema_state_dict()
     if not master_only or rank == 0:
         os.makedirs(os.path.dirname(os.path.abspath(ckpt_path)), exist_ok=True)
         tmp = ckpt_path + ".tmp"
@@ -38,6 +41,12 @@ def load_ckpt(ckpt_path: str, model, optimizer, lr_scheduler) -> None:
         model.load_state_dict(ckpt["model"], shard_metadata=ckpt.get("shard_metadata"))
     except TypeError:  # a plain nn.Module-style model
         model.load_state_dict(ckpt["model"])
+    if getattr(model, "has_ema", False):  # a model_ema in a checkpoint is ignored when the model keeps no EMA
+        if "model_ema" in ckpt:
+            model.load_ema_state_dict(ckpt["model_ema"])
+        else:
+            model.reset_ema()
+            print("the checkpoint has no model_ema: the model EMA starts from the restored weights\n", end="")
     optimizer.load_state_dict(ckpt["optimizer"])
     if getattr(model, "step_count", None) == 0 and hasattr(optimizer, "state") and hasattr(model, "all_units"):
         # DDP checkpoints carry no shard metadata: the optimizer step count is the number of steps taken
