@@ -498,8 +498,11 @@ bool make_adam(const OptT& hi, const OptT& lo, const OptT& m, const OptT& v, con
     a.v = f32_ptr(*v);
     a.lr = (float)hyper[0], a.beta1 = (float)hyper[1], a.beta2 = (float)hyper[2], a.eps = (float)hyper[3];
     a.wd = (float)hyper[4];
-    a.inv_bc1 = 1.f / (1.f - powf(a.beta1, (float)hyper[5]));
-    a.inv_bc2 = 1.f / (1.f - powf(a.beta2, (float)hyper[5]));
+    // 1 - beta^t in double, as adamw_split does: in fp32, 1 - powf(0.999f, 2) keeps only the rounding error of powf
+    // (several ulps of 0.002)
+    const double step = hyper[5];
+    a.inv_bc1 = 1.f / static_cast<float>(1.0 - std::pow(static_cast<double>(a.beta1), step));
+    a.inv_bc2 = 1.f / static_cast<float>(1.0 - std::pow(static_cast<double>(a.beta2), step));
     return true;
 }
 inline uint32_t* seq_ptr(const OptT& t) {

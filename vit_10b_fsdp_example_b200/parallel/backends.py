@@ -262,7 +262,9 @@ class Sm100Backend(TorchDistBackend):
         esize = shard.element_size()
         key = ("flags", full_buf.data_ptr(), name)
         if key not in self._seg_cache:
-            self._seg_cache[key] = torch.zeros(16, dtype=torch.int32, device=self.device)
+            # one arrival counter per slab, then the chunk counter of the copier warps at [world] (gemm_sm90.cu zeroes
+            # world + 1 words before every launch)
+            self._seg_cache[key] = torch.zeros(self.world + 1, dtype=torch.int32, device=self.device)
         flags = self._seg_cache[key]
         peers = [p + g.shard_offset * esize for p in self._peer[shard.data_ptr()]]
         return [self.world, self.rank, spec.shape[0] // self.world, g.shard_len * esize,
