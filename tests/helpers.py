@@ -1,6 +1,9 @@
 """Shared helpers for the CPU test-suite."""
+import hashlib
 import os
+import re
 import socket
+import subprocess
 import sys
 
 import torch
@@ -19,6 +22,19 @@ def tiny_cfg(**kw):
     d = dict(TINY)
     d.update(kw)
     return ViTConfig(**d)
+
+
+def sass_symbol_key(name):
+    """A kernel symbol without its anonymous-namespace tag: nvcc derives `_GLOBAL__N__<hash>_<len><file>_<hash>` from
+    the source file's path, so the same kernel has another mangled name in every checkout."""
+    return re.sub(r"_GLOBAL__N__[0-9a-f]+_(\d+)(\w*?)_[0-9a-f]{8}", r"_GLOBAL__N__\1\2", name)
+
+
+def sass_hash(obj, name):
+    """SHA-256 of kernel `name`'s SASS in object `obj` (cuobjdump), instructions only, without their addresses."""
+    out = subprocess.run(["cuobjdump", "-sass", "-fun", name, obj], capture_output=True, text=True, check=True).stdout
+    ins = [re.sub(r"/\*[0-9a-f]{4,}\*/", "", ln).strip() for ln in out.splitlines() if ";" in ln]
+    return hashlib.sha256("\n".join(ins).encode()).hexdigest()
 
 
 def free_port():

@@ -16,7 +16,7 @@ import torch
 import torch.nn.functional as F
 
 from dist_worker import launch
-from helpers import full_grads_of, full_params_of, tiny_cfg
+from helpers import full_grads_of, full_params_of, sass_hash, sass_symbol_key, tiny_cfg
 from vit_10b_fsdp_example_b200.config import ViTConfig, parse_args
 from vit_10b_fsdp_example_b200.consolidate_sharded_ckpts import consolidate_files
 from vit_10b_fsdp_example_b200.models import vit
@@ -501,20 +501,6 @@ NVCC = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc
 GOLDEN = os.path.join(ROOT, "tests", "golden", "sass_before_swiglu.json")
 
 
-def _symbol_key(name):
-    """A kernel symbol without its anonymous-namespace tag: nvcc derives `_GLOBAL__N__<hash>_<len><file>_<hash>` from
-    the source file's path, so the same kernel has another mangled name in every checkout."""
-    return re.sub(r"_GLOBAL__N__[0-9a-f]+_(\d+)(\w*?)_[0-9a-f]{8}", r"_GLOBAL__N__\1\2", name)
-
-
-def _sass_hash(obj, name):
-    import hashlib
-
-    out = subprocess.run(["cuobjdump", "-sass", "-fun", name, obj], capture_output=True, text=True, check=True).stdout
-    ins = [re.sub(r"/\*[0-9a-f]{4,}\*/", "", ln).strip() for ln in out.splitlines() if ";" in ln]
-    return hashlib.sha256("\n".join(ins).encode()).hexdigest()
-
-
 @pytest.mark.skipif(not os.path.exists(NVCC), reason="needs nvcc")
 @pytest.mark.parametrize("src,new", [("gemm_sm90.cu", ("gemm_glu_sm90_kernel",)),
                                      ("elementwise.cu", ("swiglu_fwd_kernel", "swiglu_bwd_kernel"))])
@@ -545,7 +531,7 @@ def test_kernels_compile_for_sm90a_without_spills_and_leave_existing_sass_unchan
     ver = subprocess.run([NVCC, "--version"], capture_output=True, text=True).stdout.strip().splitlines()[-1]
     if ver != golden["nvcc"]:
         pytest.skip(f"the recorded SASS is from {golden['nvcc']}, this is {ver}")
-    names = {_symbol_key(n): n for n in re.findall(r"Function : (\S+)", sass)}
+    names = {sass_symbol_key(n): n for n in re.findall(r"Function : (\S+)", sass)}
     for key, h in golden["objects"][src].items():
         assert key in names, f"pre-existing kernel {key} is gone"
-        assert _sass_hash(obj, names[key]) == h, f"SASS of pre-existing kernel {key} changed"
+        assert sass_hash(obj, names[key]) == h, f"SASS of pre-existing kernel {key} changed"

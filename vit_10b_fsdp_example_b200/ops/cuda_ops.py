@@ -404,7 +404,7 @@ def dropout(x, p: float, key: int):
     xc = x.contiguous()
     assert xc.numel() % 8 == 0, "dropout kernel works on whole 16-byte vectors"
     y = torch.empty_like(xc)
-    _C.dropout(xc, y, float(p), int(key) & 0x7FFFFFFFFFFFFFFF)
+    _C.dropout(xc, y, float(p), _drop_key(key))
     return y
 
 
@@ -508,10 +508,8 @@ def attention_fwd_lse(qkv, B: int, N: int, H: int, hd: int, drop=None):
     probability buffer of the un-fused path; lse stays that of the undropped scores."""
     out = torch.empty(B * N, H * hd, dtype=qkv.dtype, device=qkv.device)
     lse = torch.empty(B * H, N, dtype=torch.float32, device=qkv.device)
-    if drop is None:
-        _C.attention_fwd(qkv, out, lse, None, B, N, H, hd)
-    else:
-        _C.attention_fwd(qkv, out, lse, None, B, N, H, hd, float(drop[0]), _drop_key(drop[1]))
+    p, key = drop if drop is not None else (0.0, 0)
+    _C.attention_fwd(qkv, out, lse, None, B, N, H, hd, float(p), _drop_key(key))
     return out, lse
 
 
@@ -521,10 +519,8 @@ def attention_bwd_lse(dout, qkv, out, lse, B: int, N: int, H: int, hd: int, want
     delta = torch.empty(B * H, N, dtype=torch.float32, device=qkv.device)  # scratch: rowsum(dO o O)
     # the backward kernels reduce the qkv bias gradient (column sums of dq | dk | dv) from their epilogue tiles
     cs = torch.zeros(3 * H * hd, dtype=torch.float32, device=qkv.device) if want_colsum else None
-    if drop is None:
-        _C.attention_bwd(qkv, dout, out, lse, delta, dqkv, cs, B, N, H, hd)
-    else:
-        _C.attention_bwd(qkv, dout, out, lse, delta, dqkv, cs, B, N, H, hd, float(drop[0]), _drop_key(drop[1]))
+    p, key = drop if drop is not None else (0.0, 0)
+    _C.attention_bwd(qkv, dout, out, lse, delta, dqkv, cs, B, N, H, hd, float(p), _drop_key(key))
     return (dqkv, cs) if want_colsum else dqkv
 
 
@@ -567,7 +563,7 @@ def attention_bwd(dout, qkv, p, B: int, N: int, H: int, hd: int, want_colsum: bo
         dp[:, :, N:].zero_()
     gemm_raw(dout, ldo, 0, v, ld3, 0, dp, ldp, N, N, hd, batch=(H, B, *bo, *bq, *bp))
     if drop is not None:
-        _C.dropout(dp, dp, float(drop[0]), int(drop[1]) & 0x7FFFFFFFFFFFFFFF)  # same key and shape -> same mask
+        _C.dropout(dp, dp, float(drop[0]), _drop_key(drop[1]))  # same key and shape -> same mask
     # dS = scale * P * (dP - rowsum(dP * P))   (in place)
     _C.softmax_bwd(dp, p, B * H * N, N, ldp, hd ** -0.5)
     # dQ = dS K ; dK = dS^T Q
