@@ -65,6 +65,9 @@ struct GemmAgFuse {
 // D[b][M, N] = epi(A[b] (M x K) * B[b] (N x K)^T).  major_x: 0 = K contiguous, 1 = M/N contiguous.
 // block_n: 0 = auto, else 128 / 256.  cluster: 0 = auto (= 1), 1 = one CTA per tile, 2 = CTA pairs along M sharing
 // B through TMA multicast (1 is used when max_ctas = 1).  max_ctas: 0 = all SMs (used to carve SMs out for comm kernels).
+// With N % 8 != 0 the TMA store writes whole 16-byte units, so the columns [N, pad8(N)) of every row are written too:
+// with +0 in D, with unspecified values in the aux output.  Every ld is a multiple of 8, so this stays inside the row,
+// but a D or aux output that is a column slice of a wider matrix must leave those columns to the GEMM.
 void gemm_bf16(const GemmOperand& A, int major_a, const GemmOperand& B, int major_b, const GemmOperand& D,
                const GemmOperand* aux_out, int M, int N, int K, const GemmEpilogue& epi, int block_n, int cluster,
                int max_ctas, cudaStream_t stream, const GemmAgFuse* ag = nullptr);
