@@ -118,6 +118,16 @@ def build_arg_parser() -> argparse.ArgumentParser:
     parser.add_argument("--model_ema_decay", type=_ema_decay, default=0.9998,
                         help="EMA decay d: ema = d * ema + (1 - d) * w after every step (timm train.py 0.9998, DeiT "
                              "0.99996); in [0, 1), 0 = the EMA is the weights")
+    # ---- optimizer parameter groups (MAE param_groups_lrd; timm create_optimizer_v2 filter_bias_and_bn / --layer-decay) ----
+    parser.add_argument("--filter_bias_and_norm", action="store_true",
+                        help="no weight decay on parameters that are 1-D in timm's layout (biases, LayerNorm and q/k "
+                             "norm weights, LayerScale gammas) nor on pos_embed, cls_token and reg_token (timm "
+                             "filter_bias_and_bn, DeiT, MAE); off = decay every tensor like the reference")
+    parser.add_argument("--layer_decay", type=_layer_decay, default=None,
+                        help="layer-wise lr decay d (BEiT / MAE / DINOv2 fine-tuning, timm --layer-decay): block i trains "
+                             "at lr * d ** (num_blocks - i), the stem (patch_embed, pos_embed, tokens) at "
+                             "lr * d ** (num_blocks + 1), the final norm and head at lr; in (0, 1], typically 0.65-0.75; "
+                             "implies --filter_bias_and_norm (1 = the filter alone)")
     return parser
 
 
@@ -157,6 +167,13 @@ def _ema_decay(s: str) -> float:
     v = float(s)
     if not 0.0 <= v < 1.0:
         raise argparse.ArgumentTypeError(f"--model_ema_decay must be in [0, 1), got {s}")
+    return v
+
+
+def _layer_decay(s: str) -> float:
+    v = float(s)
+    if not 0.0 < v <= 1.0:
+        raise argparse.ArgumentTypeError(f"--layer_decay must be in (0, 1], got {s}")
     return v
 
 

@@ -407,10 +407,27 @@ void sumsq(Tensor x, Tensor out) {
     b200::sumsq(x.data_ptr(), is_bf16, x.numel(), f32_ptr(out), cur_stream());
 }
 
+// Parameter groups of the grouped AdamW kernels: `groups` uint8 [n / 64] (the group of every 64-element chunk),
+// `group_hyper` fp32 [G, 2] rows of (lr_scale, wd); both or neither.  Returns false when neither is given.
+bool check_groups(const char* who, const OptT& groups, const OptT& group_hyper, int64_t n, const at::Device& dev) {
+    TORCH_CHECK(groups.has_value() == group_hyper.has_value(), who, ": pass both groups and group_hyper, or neither");
+    if (!groups.has_value()) return false;
+    TORCH_CHECK(groups->scalar_type() == at::kByte && group_hyper->scalar_type() == at::kFloat, who,
+                ": groups must be uint8 and group_hyper fp32");
+    TORCH_CHECK(groups->device() == dev && group_hyper->device() == dev && groups->is_contiguous() &&
+                    group_hyper->is_contiguous(), who, ": groups and group_hyper must be contiguous, on the shard's device");
+    TORCH_CHECK(n % 64 == 0 && groups->numel() == n / 64, who, ": ", n, " elements need n % 64 == 0 and n / 64 chunk "
+                "groups, got ", groups->numel());
+    TORCH_CHECK(group_hyper->dim() == 2 && group_hyper->size(1) == 2 && group_hyper->size(0) >= 1 &&
+                    group_hyper->size(0) <= 256, who, ": group_hyper must be [G, 2] with 1 <= G <= 256");
+    return true;
+}
+
 void adamw_split(Tensor hi, Tensor lo, Tensor m, Tensor v, Tensor grad, OptT clip_coef, double lr, double beta1,
                  double beta2, double eps, double wd, int64_t step, OptT hyper, OptT ema_hi, OptT ema_lo,
-                 double ema_decay) {
+                 double ema_decay, OptT groups, OptT group_hyper) {
     c10::cuda::CUDAGuard guard(hi.device());
+    const bool grouped = check_groups("adamw_split", groups, group_hyper, hi.numel(), hi.device());
     TORCH_CHECK(hi.scalar_type() == at::kBFloat16 && lo.scalar_type() == at::kShort, "hi: bf16, lo: int16");
     TORCH_CHECK(ema_hi.has_value() == ema_lo.has_value(), "adamw_split: pass both ema_hi and ema_lo, or neither");
     if (ema_hi.has_value()) {
@@ -428,12 +445,14 @@ void adamw_split(Tensor hi, Tensor lo, Tensor m, Tensor v, Tensor grad, OptT cli
                       clip_coef.has_value() ? f32_ptr(*clip_coef) : nullptr, (float)lr, (float)beta1, (float)beta2,
                       (float)eps, (float)wd, (int)step, cur_stream(), hyper.has_value() ? f32_ptr(*hyper) : nullptr,
                       ema_hi.has_value() ? reinterpret_cast<uint16_t*>(ema_hi->data_ptr()) : nullptr,
-                      ema_lo.has_value() ? reinterpret_cast<int16_t*>(ema_lo->data_ptr()) : nullptr, (float)ema_decay);
+                      ema_lo.has_value() ? reinterpret_cast<int16_t*>(ema_lo->data_ptr()) : nullptr, (float)ema_decay,
+                      grouped ? groups->data_ptr<uint8_t>() : nullptr, grouped ? f32_ptr(*group_hyper) : nullptr);
 }
 
 void adamw_fp32(Tensor w, Tensor m, Tensor v, Tensor grad, OptT clip_coef, double lr, double beta1, double beta2,
-                double eps, double wd, int64_t step, OptT ema, double ema_decay) {
+                double eps, double wd, int64_t step, OptT ema, double ema_decay, OptT groups, OptT group_hyper) {
     c10::cuda::CUDAGuard guard(w.device());
+    const bool grouped = check_groups("adamw_fp32", groups, group_hyper, w.numel(), w.device());
     if (ema.has_value()) {
         TORCH_CHECK(ema->scalar_type() == at::kFloat && ema->numel() == w.numel() && ema->is_contiguous() &&
                         ema->device() == w.device(), "adamw_fp32: the EMA must be a contiguous fp32 tensor like w");
@@ -443,7 +462,8 @@ void adamw_fp32(Tensor w, Tensor m, Tensor v, Tensor grad, OptT clip_coef, doubl
     b200::adamw_fp32(f32_ptr(w), f32_ptr(m), f32_ptr(v), grad.data_ptr(), gbf, w.numel(),
                      clip_coef.has_value() ? f32_ptr(*clip_coef) : nullptr, (float)lr, (float)beta1, (float)beta2,
                      (float)eps, (float)wd, (int)step, cur_stream(), ema.has_value() ? f32_ptr(*ema) : nullptr,
-                     (float)ema_decay);
+                     (float)ema_decay, grouped ? groups->data_ptr<uint8_t>() : nullptr,
+                     grouped ? f32_ptr(*group_hyper) : nullptr);
 }
 
 void split_fp32(Tensor w, Tensor hi, Tensor lo) {
@@ -525,10 +545,16 @@ bool make_sync(const std::vector<int64_t>& sync, const std::vector<int64_t>& fla
 void reduce_scatter(std::vector<int64_t> peer_ptrs, int64_t mc_ptr, int64_t rank, int64_t world, Tensor out,
                     Tensor seg_table, int64_t total_chunks, bool in_is_bf16, double scale, OptT sumsq_out,
                     int64_t max_ctas, std::vector<int64_t> sync, std::vector<int64_t> flag_ptrs, OptT seq_dev,
-                    OptT cta_ctr, OptT hi, OptT lo, OptT m, OptT v, std::vector<double> hyper) {
+                    OptT cta_ctr, OptT hi, OptT lo, OptT m, OptT v, std::vector<double> hyper, OptT groups,
+                    OptT group_hyper) {
     c10::cuda::CUDAGuard guard(out.device());
     b200::AdamFuse a;
     const bool fused = make_adam(hi, lo, m, v, hyper, a);
+    TORCH_CHECK(fused || !groups.has_value(), "reduce_scatter: parameter groups need the fused-AdamW arguments");
+    if (fused && check_groups("reduce_scatter", groups, group_hyper, hi->numel(), hi->device())) {
+        a.groups = groups->data_ptr<uint8_t>();
+        a.group_hyper = f32_ptr(*group_hyper);
+    }
     b200::CommSync cs;
     const bool synced = make_sync(sync, flag_ptrs, seq_dev, cta_ctr, cs);
     b200::reduce_scatter(peer_ptrs, mc_ptr, (int)rank, (int)world, f32_ptr(out), seg_ptr(seg_table),
@@ -605,16 +631,22 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("adamw_split", &adamw_split, py::arg("hi"), py::arg("lo"), py::arg("m"), py::arg("v"), py::arg("grad"),
           py::arg("clip_coef"), py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"),
           py::arg("step"), py::arg("hyper") = py::none(), py::arg("ema_hi") = py::none(),
-          py::arg("ema_lo") = py::none(), py::arg("ema_decay") = 0.0);
+          py::arg("ema_lo") = py::none(), py::arg("ema_decay") = 0.0, py::arg("groups") = py::none(),
+          py::arg("group_hyper") = py::none());
     m.def("adamw_fp32", &adamw_fp32, py::arg("w"), py::arg("m"), py::arg("v"), py::arg("grad"), py::arg("clip_coef"),
           py::arg("lr"), py::arg("beta1"), py::arg("beta2"), py::arg("eps"), py::arg("wd"), py::arg("step"),
-          py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0);
+          py::arg("ema") = py::none(), py::arg("ema_decay") = 0.0, py::arg("groups") = py::none(),
+          py::arg("group_hyper") = py::none());
     m.def("split_fp32", &split_fp32);
     m.def("merge_fp32", &merge_fp32);
     m.def("clip_coef", &clip_coef);
     m.def("p2p_all_gather", &p2p_all_gather);
     m.def("ce_all_gather", &ce_all_gather);
-    m.def("reduce_scatter", &reduce_scatter);
+    m.def("reduce_scatter", &reduce_scatter, py::arg("peer_ptrs"), py::arg("mc_ptr"), py::arg("rank"), py::arg("world"),
+          py::arg("out"), py::arg("seg_table"), py::arg("total_chunks"), py::arg("in_is_bf16"), py::arg("scale"),
+          py::arg("sumsq_out"), py::arg("max_ctas"), py::arg("sync"), py::arg("flag_ptrs"), py::arg("seq_dev"),
+          py::arg("cta_ctr"), py::arg("hi"), py::arg("lo"), py::arg("m"), py::arg("v"), py::arg("hyper"),
+          py::arg("groups") = py::none(), py::arg("group_hyper") = py::none());
     m.def("all_reduce_mean", &all_reduce_mean);
     m.def("rs_chunk_vecs", &rs_chunk_vecs);
     m.def("signal_barrier", &signal_barrier);

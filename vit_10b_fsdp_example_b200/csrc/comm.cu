@@ -306,7 +306,12 @@ __global__ void __launch_bounds__(kCommThreads, kNvls && !kAdam ? 8 : 5)
                 if constexpr (kAdam) {
                     // Sharded AdamW right here: the reduced gradient never goes to memory.
                     const int64_t e = row[1] + (v0 + i) * kVec;  // element offset inside the shard
-                    const float decay = 1.f - adam.lr * adam.wd;
+                    float lr = adam.lr, decay = 1.f - adam.lr * adam.wd;
+                    if (adam.groups != nullptr) {  // a vector of kVec elements never crosses a 64-element chunk
+                        const int grp = adam.groups[e >> 6];
+                        lr = adam.lr * __ldg(adam.group_hyper + 2 * grp);
+                        decay = 1.f - lr * __ldg(adam.group_hyper + 2 * grp + 1);
+                    }
 #pragma unroll
                     for (int q = 0; q < kVec; ++q) {
                         const int32_t bits =
@@ -317,7 +322,7 @@ __global__ void __launch_bounds__(kCommThreads, kNvls && !kAdam ? 8 : 5)
                         const float vi = adam.beta2 * adam.v[e + q] + (1.f - adam.beta2) * g * g;
                         adam.m[e + q] = mi;
                         adam.v[e + q] = vi;
-                        w = w * decay - adam.lr * (mi * adam.inv_bc1) / (sqrtf(vi * adam.inv_bc2) + adam.eps);
+                        w = w * decay - lr * (mi * adam.inv_bc1) / (sqrtf(vi * adam.inv_bc2) + adam.eps);
                         const int32_t nb = __float_as_int(w);
                         const int32_t h = (nb + 0x8000) >> 16;
                         adam.hi[e + q] = static_cast<uint16_t>(h & 0xFFFF);
@@ -490,6 +495,8 @@ void reduce_scatter(const std::vector<int64_t>& peer_ptrs, int64_t mc_ptr, int r
     const bool nvls = mc_ptr != 0;
     if (nvls && !in_is_bf16) throw std::runtime_error("reduce_scatter: the in-switch reduction path is bf16 only");
     if (adam != nullptr && !in_is_bf16) throw std::runtime_error("reduce_scatter: fused AdamW needs bf16 gradients");
+    if (adam != nullptr && (adam->groups == nullptr) != (adam->group_hyper == nullptr))
+        throw std::runtime_error("reduce_scatter: the parameter groups need both groups and group_hyper (or neither)");
     const SyncArgs ks = to_sync(sync);  // world <= 1 in there: no flag protocol (caller brackets with barriers)
     const PeerPtrs peers = nvls ? PeerPtrs{} : to_peers(peer_ptrs);
     const uint64_t mc = static_cast<uint64_t>(mc_ptr);

@@ -20,6 +20,10 @@ struct AdamFuse {
     float* m = nullptr;
     float* v = nullptr;
     float lr = 0.f, beta1 = 0.9f, beta2 = 0.999f, eps = 1e-8f, wd = 0.f, inv_bc1 = 1.f, inv_bc2 = 1.f;
+    // parameter groups (optional): groups[e / 64] is the group of shard element e, group_hyper its fp32 row
+    // (lr_scale, wd); the update then uses lr * lr_scale and that wd.  Null = one group (lr, wd).
+    const uint8_t* groups = nullptr;
+    const float* group_hyper = nullptr;
 };
 // Cross-GPU flag protocol folded into reduce_scatter / all_reduce (no separate barrier launches): "inputs ready"
 // flags are published at kernel start, "done reading" flags by the last CTA, which also waits for every peer's.

@@ -1083,14 +1083,20 @@ __device__ __forceinline__ void split_bits(float w, uint32_t& h_out, uint32_t& l
 // ema_hi (bf16) + ema_lo (int16), and updated from the new fp32 w while it is still in registers:
 //   ema = fmaf(d, ema, (1 - d) * w)        (1 - d formed in fp32, so d = 0 gives ema == w bitwise)
 // 8 more bytes per element (ema_hi + ema_lo, read and written); hi / lo / m / v are computed exactly as without it.
-template <typename GradT, bool EMA>
+// GROUPED (parameter groups, see parallel/param_groups.py): every 64-element chunk i >> 6 of the shard belongs to group
+// groups[i >> 6], whose row of group_hyper is (lr_scale, wd).  A 4-element vector never crosses a chunk, so each reads
+// its group once and uses lr * lr_scale and 1 - lr * lr_scale * wd, formed in fp32, in place of lr and 1 - lr * wd.
+// One byte of traffic per 64 elements; the arithmetic is otherwise the ungrouped kernel's.
+template <typename GradT, bool EMA, bool GROUPED = false>
 __device__ __forceinline__ void adamw_split_body(uint16_t* __restrict__ hi, int16_t* __restrict__ lo,
                                                  float* __restrict__ m, float* __restrict__ v,
                                                  const GradT* __restrict__ grad, int64_t n,
                                                  const float* __restrict__ clip_coef, float lr, float beta1, float beta2,
                                                  float eps, float wd, float bc1, float bc2,
                                                  const float* __restrict__ hyper, uint16_t* __restrict__ ema_hi,
-                                                 int16_t* __restrict__ ema_lo, float ema_decay) {
+                                                 int16_t* __restrict__ ema_lo, float ema_decay,
+                                                 const uint8_t* __restrict__ groups = nullptr,
+                                                 const float* __restrict__ group_hyper = nullptr) {
     const float coef = clip_coef != nullptr ? *clip_coef : 1.0f;
     if (hyper != nullptr) {  // lr and step live on the device so the launch can sit inside a CUDA graph
         lr = hyper[0];
@@ -1121,6 +1127,12 @@ __device__ __forceinline__ void adamw_split_body(uint16_t* __restrict__ hi, int1
         const uint32_t lw[4] = {lv.x & 0xFFFFu, lv.x >> 16, lv.y & 0xFFFFu, lv.y >> 16};
         float mm[4] = {mv.x, mv.y, mv.z, mv.w}, vq[4] = {vv.x, vv.y, vv.z, vv.w};
         uint32_t ho[4], lo_o[4], eho[4], elo[4];
+        float lr_q = lr, decay_q = decay;
+        if constexpr (GROUPED) {
+            const int grp = groups[i >> 6];
+            lr_q = lr * __ldg(group_hyper + 2 * grp);
+            decay_q = 1.f - lr_q * __ldg(group_hyper + 2 * grp + 1);
+        }
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             const int32_t bits = static_cast<int32_t>(hw[k] << 16) + static_cast<int32_t>(static_cast<int16_t>(lw[k]));
@@ -1128,7 +1140,7 @@ __device__ __forceinline__ void adamw_split_body(uint16_t* __restrict__ hi, int1
             const float gk = g[k] * coef;
             mm[k] = beta1 * mm[k] + (1.f - beta1) * gk;
             vq[k] = beta2 * vq[k] + (1.f - beta2) * gk * gk;
-            w = w * decay - lr * (mm[k] * inv_bc1) / (sqrtf(vq[k] * inv_bc2) + eps);
+            w = w * decay_q - lr_q * (mm[k] * inv_bc1) / (sqrtf(vq[k] * inv_bc2) + eps);
             const int32_t nb = __float_as_int(w);
             const int32_t rounded = nb + 0x8000;  // round-half-up: keeps lo in [-32768, 32767] (see split_fp32)
             const int32_t h = rounded >> 16;
@@ -1150,7 +1162,8 @@ __device__ __forceinline__ void adamw_split_body(uint16_t* __restrict__ hi, int1
             *reinterpret_cast<uint2*>(ema_lo + i) = make_uint2(elo[0] | (elo[1] << 16), elo[2] | (elo[3] << 16));
         }
     }
-    // scalar tail (n not a multiple of 4)
+    // scalar tail (n not a multiple of 4; never taken by the grouped kernels, whose n is a multiple of 64)
+    if constexpr (GROUPED) return;
     for (int64_t i = n4 * 4 + static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
          i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
         const int32_t bits = (static_cast<int32_t>(hi[i]) << 16) + static_cast<int32_t>(lo[i]);
@@ -1200,13 +1213,36 @@ __global__ void __launch_bounds__(256) adamw_split_ema_kernel(uint16_t* __restri
                                   ema_hi, ema_lo, ema_decay);
 }
 
+// Parameter-group variants of the two kernels above (n % 64 == 0).
+template <typename GradT>
+__global__ void __launch_bounds__(256) adamw_split_grouped_kernel(
+    uint16_t* __restrict__ hi, int16_t* __restrict__ lo, float* __restrict__ m, float* __restrict__ v,
+    const GradT* __restrict__ grad, int64_t n, const float* __restrict__ clip_coef, float lr, float beta1, float beta2,
+    float eps, float bc1, float bc2, const float* __restrict__ hyper, const uint8_t* __restrict__ groups,
+    const float* __restrict__ group_hyper) {
+    adamw_split_body<GradT, false, true>(hi, lo, m, v, grad, n, clip_coef, lr, beta1, beta2, eps, 0.f, bc1, bc2, hyper,
+                                         nullptr, nullptr, 0.f, groups, group_hyper);
+}
+
+template <typename GradT>
+__global__ void __launch_bounds__(256) adamw_split_ema_grouped_kernel(
+    uint16_t* __restrict__ hi, int16_t* __restrict__ lo, float* __restrict__ m, float* __restrict__ v,
+    const GradT* __restrict__ grad, int64_t n, const float* __restrict__ clip_coef, float lr, float beta1, float beta2,
+    float eps, float bc1, float bc2, const float* __restrict__ hyper, uint16_t* __restrict__ ema_hi,
+    int16_t* __restrict__ ema_lo, float ema_decay, const uint8_t* __restrict__ groups,
+    const float* __restrict__ group_hyper) {
+    adamw_split_body<GradT, true, true>(hi, lo, m, v, grad, n, clip_coef, lr, beta1, beta2, eps, 0.f, bc1, bc2, hyper,
+                                        ema_hi, ema_lo, ema_decay, groups, group_hyper);
+}
+
 // Plain fp32-master variant (used when the compute dtype is fp32); the EMA is a plain fp32 shard here.
-template <typename GradT, bool EMA>
+template <typename GradT, bool EMA, bool GROUPED = false>
 __device__ __forceinline__ void adamw_fp32_body(float* __restrict__ w, float* __restrict__ m, float* __restrict__ v,
                                                 const GradT* __restrict__ grad, int64_t n,
                                                 const float* __restrict__ clip_coef, float lr, float beta1, float beta2,
                                                 float eps, float wd, float bc1, float bc2, float* __restrict__ ema,
-                                                float ema_decay) {
+                                                float ema_decay, const uint8_t* __restrict__ groups = nullptr,
+                                                const float* __restrict__ group_hyper = nullptr) {
     const float coef = clip_coef != nullptr ? *clip_coef : 1.0f;
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
          i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
@@ -1215,7 +1251,13 @@ __device__ __forceinline__ void adamw_fp32_body(float* __restrict__ w, float* __
         const float vi = beta2 * v[i] + (1.f - beta2) * g * g;
         m[i] = mi;
         v[i] = vi;
-        const float wi = w[i] * (1.f - lr * wd) - lr * (mi / bc1) / (sqrtf(vi / bc2) + eps);
+        float lr_i = lr, wd_i = wd;
+        if constexpr (GROUPED) {
+            const int grp = groups[i >> 6];
+            lr_i = lr * __ldg(group_hyper + 2 * grp);
+            wd_i = __ldg(group_hyper + 2 * grp + 1);
+        }
+        const float wi = w[i] * (1.f - lr_i * wd_i) - lr_i * (mi / bc1) / (sqrtf(vi / bc2) + eps);
         w[i] = wi;
         if constexpr (EMA) ema[i] = fmaf(ema_decay, ema[i], (1.f - ema_decay) * wi);
     }
@@ -1237,6 +1279,24 @@ __global__ void __launch_bounds__(256) adamw_fp32_ema_kernel(float* __restrict__
                                                              float beta1, float beta2, float eps, float wd, float bc1,
                                                              float bc2, float* __restrict__ ema, float ema_decay) {
     adamw_fp32_body<GradT, true>(w, m, v, grad, n, clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2, ema, ema_decay);
+}
+
+template <typename GradT>
+__global__ void __launch_bounds__(256) adamw_fp32_grouped_kernel(
+    float* __restrict__ w, float* __restrict__ m, float* __restrict__ v, const GradT* __restrict__ grad, int64_t n,
+    const float* __restrict__ clip_coef, float lr, float beta1, float beta2, float eps, float bc1, float bc2,
+    const uint8_t* __restrict__ groups, const float* __restrict__ group_hyper) {
+    adamw_fp32_body<GradT, false, true>(w, m, v, grad, n, clip_coef, lr, beta1, beta2, eps, 0.f, bc1, bc2, nullptr, 0.f,
+                                        groups, group_hyper);
+}
+
+template <typename GradT>
+__global__ void __launch_bounds__(256) adamw_fp32_ema_grouped_kernel(
+    float* __restrict__ w, float* __restrict__ m, float* __restrict__ v, const GradT* __restrict__ grad, int64_t n,
+    const float* __restrict__ clip_coef, float lr, float beta1, float beta2, float eps, float bc1, float bc2,
+    float* __restrict__ ema, float ema_decay, const uint8_t* __restrict__ groups, const float* __restrict__ group_hyper) {
+    adamw_fp32_body<GradT, true, true>(w, m, v, grad, n, clip_coef, lr, beta1, beta2, eps, 0.f, bc1, bc2, ema, ema_decay,
+                                       groups, group_hyper);
 }
 
 // Split an fp32 tensor into (hi bf16, lo int16) and back.
@@ -1577,15 +1637,36 @@ void sumsq(const void* x, bool is_bf16, int64_t n, float* out, cudaStream_t stre
 
 void adamw_split(uint16_t* hi, int16_t* lo, float* m, float* v, const void* grad, bool grad_is_bf16, int64_t n,
                  const float* clip_coef, float lr, float beta1, float beta2, float eps, float wd, int step,
-                 cudaStream_t stream, const float* hyper, uint16_t* ema_hi, int16_t* ema_lo, float ema_decay) {
+                 cudaStream_t stream, const float* hyper, uint16_t* ema_hi, int16_t* ema_lo, float ema_decay,
+                 const uint8_t* groups, const float* group_hyper) {
     if ((ema_hi == nullptr) != (ema_lo == nullptr))
         throw std::runtime_error("adamw_split: the EMA needs both ema_hi and ema_lo (or neither)");
+    if ((groups == nullptr) != (group_hyper == nullptr))
+        throw std::runtime_error("adamw_split: the parameter groups need both groups and group_hyper (or neither)");
+    if (groups != nullptr && n % 64 != 0) throw std::runtime_error("adamw_split: grouped update needs n % 64 == 0");
     const int grid = static_cast<int>(std::min<int64_t>((n / 4 + 255) / 256 + 1, sm_count() * 16));
     if (grid == 0) return;
     // 1 - beta^t in double: in fp32, 1 - powf(0.999f, 2) keeps only the rounding error of powf (1.5e-5 of 0.002)
     const float bc1 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta1), static_cast<double>(step)));
     const float bc2 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta2), static_cast<double>(step)));
-    if (ema_hi != nullptr) {
+    if (groups != nullptr) {
+        if (ema_hi != nullptr && grad_is_bf16)
+            adamw_split_ema_grouped_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
+                hi, lo, m, v, static_cast<const __nv_bfloat16*>(grad), n, clip_coef, lr, beta1, beta2, eps, bc1, bc2,
+                hyper, ema_hi, ema_lo, ema_decay, groups, group_hyper);
+        else if (ema_hi != nullptr)
+            adamw_split_ema_grouped_kernel<float><<<grid, 256, 0, stream>>>(
+                hi, lo, m, v, static_cast<const float*>(grad), n, clip_coef, lr, beta1, beta2, eps, bc1, bc2, hyper,
+                ema_hi, ema_lo, ema_decay, groups, group_hyper);
+        else if (grad_is_bf16)
+            adamw_split_grouped_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
+                hi, lo, m, v, static_cast<const __nv_bfloat16*>(grad), n, clip_coef, lr, beta1, beta2, eps, bc1, bc2,
+                hyper, groups, group_hyper);
+        else
+            adamw_split_grouped_kernel<float><<<grid, 256, 0, stream>>>(
+                hi, lo, m, v, static_cast<const float*>(grad), n, clip_coef, lr, beta1, beta2, eps, bc1, bc2, hyper,
+                groups, group_hyper);
+    } else if (ema_hi != nullptr) {
         if (grad_is_bf16)
             adamw_split_ema_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
                 hi, lo, m, v, static_cast<const __nv_bfloat16*>(grad), n, clip_coef, lr, beta1, beta2, eps, wd, bc1,
@@ -1607,13 +1688,33 @@ void adamw_split(uint16_t* hi, int16_t* lo, float* m, float* v, const void* grad
 
 void adamw_fp32(float* w, float* m, float* v, const void* grad, bool grad_is_bf16, int64_t n, const float* clip_coef,
                 float lr, float beta1, float beta2, float eps, float wd, int step, cudaStream_t stream, float* ema,
-                float ema_decay) {
+                float ema_decay, const uint8_t* groups, const float* group_hyper) {
+    if ((groups == nullptr) != (group_hyper == nullptr))
+        throw std::runtime_error("adamw_fp32: the parameter groups need both groups and group_hyper (or neither)");
+    if (groups != nullptr && n % 64 != 0) throw std::runtime_error("adamw_fp32: grouped update needs n % 64 == 0");
     const int grid = static_cast<int>(std::min<int64_t>((n + 255) / 256, sm_count() * 16));
     if (grid == 0) return;
     // 1 - beta^t in double: in fp32, 1 - powf(0.999f, 2) keeps only the rounding error of powf (1.5e-5 of 0.002)
     const float bc1 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta1), static_cast<double>(step)));
     const float bc2 = static_cast<float>(1.0 - std::pow(static_cast<double>(beta2), static_cast<double>(step)));
-    if (ema != nullptr) {
+    if (groups != nullptr) {
+        if (ema != nullptr && grad_is_bf16)
+            adamw_fp32_ema_grouped_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
+                w, m, v, static_cast<const __nv_bfloat16*>(grad), n, clip_coef, lr, beta1, beta2, eps, bc1, bc2, ema,
+                ema_decay, groups, group_hyper);
+        else if (ema != nullptr)
+            adamw_fp32_ema_grouped_kernel<float><<<grid, 256, 0, stream>>>(
+                w, m, v, static_cast<const float*>(grad), n, clip_coef, lr, beta1, beta2, eps, bc1, bc2, ema, ema_decay,
+                groups, group_hyper);
+        else if (grad_is_bf16)
+            adamw_fp32_grouped_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
+                w, m, v, static_cast<const __nv_bfloat16*>(grad), n, clip_coef, lr, beta1, beta2, eps, bc1, bc2, groups,
+                group_hyper);
+        else
+            adamw_fp32_grouped_kernel<float><<<grid, 256, 0, stream>>>(
+                w, m, v, static_cast<const float*>(grad), n, clip_coef, lr, beta1, beta2, eps, bc1, bc2, groups,
+                group_hyper);
+    } else if (ema != nullptr) {
         if (grad_is_bf16)
             adamw_fp32_ema_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
                 w, m, v, static_cast<const __nv_bfloat16*>(grad), n, clip_coef, lr, beta1, beta2, eps, wd, bc1, bc2, ema,

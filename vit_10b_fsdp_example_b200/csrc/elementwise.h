@@ -80,11 +80,15 @@ void sumsq(const void* x, bool is_bf16, int64_t n, float* out, cudaStream_t stre
 void adamw_split(uint16_t* hi, int16_t* lo, float* m, float* v, const void* grad, bool grad_is_bf16, int64_t n,
                  const float* clip_coef, float lr, float beta1, float beta2, float eps, float wd, int step,
                  cudaStream_t stream, const float* hyper = nullptr, uint16_t* ema_hi = nullptr,
-                 int16_t* ema_lo = nullptr, float ema_decay = 0.f);
+                 int16_t* ema_lo = nullptr, float ema_decay = 0.f, const uint8_t* groups = nullptr,
+                 const float* group_hyper = nullptr);
 // ema (optional): fp32 model EMA, same recurrence
+// groups / group_hyper (optional, device; both or neither): parameter groups.  groups[i / 64] is the group of element
+// i (n % 64 == 0), group_hyper its fp32 row (lr_scale, wd); the update uses lr * lr_scale and that wd (`wd` is unused)
 void adamw_fp32(float* w, float* m, float* v, const void* grad, bool grad_is_bf16, int64_t n, const float* clip_coef,
                 float lr, float beta1, float beta2, float eps, float wd, int step, cudaStream_t stream,
-                float* ema = nullptr, float ema_decay = 0.f);
+                float* ema = nullptr, float ema_decay = 0.f, const uint8_t* groups = nullptr,
+                const float* group_hyper = nullptr);
 void split_fp32(const float* w, uint16_t* hi, int16_t* lo, int64_t n, cudaStream_t stream);
 void merge_fp32(const uint16_t* hi, const int16_t* lo, float* w, int64_t n, cudaStream_t stream);
 void clip_coef(const float* sumsq_in, float max_norm, float* coef, float* norm_out, cudaStream_t stream);

@@ -627,20 +627,29 @@ def clip_coef(sumsq_t, max_norm: float):
     return coef, norm
 
 
-def adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, ema=None, ema_decay: float = 0.0):
-    """ema: optional fp32 model EMA, updated in the same pass as ema = fmaf(d, ema, (1 - d) * w_new)."""
-    if ema is None:
+def adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, ema=None, ema_decay: float = 0.0,
+               groups=None, group_hyper=None):
+    """ema: optional fp32 model EMA, updated in the same pass as ema = fmaf(d, ema, (1 - d) * w_new).
+    groups / group_hyper: optional parameter groups, the uint8 group of every 64-element chunk and the fp32 [G, 2]
+    rows of (lr_scale, wd); the grouped kernels then use lr * lr_scale and that wd per chunk (`wd` is unused)."""
+    if groups is not None:
+        _C.adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, ema, float(ema_decay), groups, group_hyper)
+    elif ema is None:
         _C.adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step)
     else:
         _C.adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, ema, float(ema_decay))
 
 
 def adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, hyper=None, ema=None,
-                ema_decay: float = 0.0):
+                ema_decay: float = 0.0, groups=None, group_hyper=None):
     """hyper: optional device tensor [lr, step] that overrides the host scalars (CUDA-graph replay).
     ema: optional (ema_hi, ema_lo), the model EMA in the master's split form, updated in the same pass as
-    ema = fmaf(d, ema, (1 - d) * w_new) with d = ema_decay."""
-    if ema is None:
+    ema = fmaf(d, ema, (1 - d) * w_new) with d = ema_decay.  groups / group_hyper: as in adamw_fp32."""
+    if groups is not None:
+        e_hi, e_lo = ema if ema is not None else (None, None)
+        _C.adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, hyper, e_hi, e_lo,
+                       float(ema_decay), groups, group_hyper)
+    elif ema is None:
         _C.adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, hyper)
     else:
         _C.adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, hyper, ema[0], ema[1],

@@ -547,14 +547,27 @@ def ema_update(ema, w, decay: float):
     ema.copy_((ema.double() * d + keep.double()).float())
 
 
-def adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, ema=None, ema_decay: float = 0.0):
-    """ema: optional fp32 model EMA, updated from the new w (see ema_update)."""
-    _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step)
+def adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, ema=None, ema_decay: float = 0.0,
+               groups=None, group_hyper=None):
+    """ema: optional fp32 model EMA, updated from the new w (see ema_update).
+    groups / group_hyper: optional parameter groups (see group_lr_decay); `wd` is then unused."""
+    _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, groups, group_hyper)
     if ema is not None:
         ema_update(ema, w, ema_decay)
 
 
-def _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int):
+def group_lr_decay(lr, groups, group_hyper, n: int):
+    """Per-element (lr * lr_scale, 1 - lr * lr_scale * wd) in fp32, as the grouped kernels form them: `groups` is the
+    uint8 group of every 64-element chunk, `group_hyper` the fp32 [G, 2] rows of (lr_scale, wd)."""
+    if n != groups.numel() * 64:
+        raise ValueError(f"grouped AdamW: {n} elements need {n // 64} chunk groups (n % 64 == 0), got {groups.numel()}")
+    gh = group_hyper.to(device=groups.device, dtype=torch.float32)
+    idx = groups.long().repeat_interleave(64)
+    lr_e = gh[idx, 0] * torch.tensor(lr, dtype=torch.float32, device=groups.device)
+    return lr_e, 1.0 - lr_e * gh[idx, 1]
+
+
+def _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, groups=None, group_hyper=None):
     g = _f32(grad)
     if clip is not None:
         g = g * clip
@@ -562,9 +575,14 @@ def _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int):
     v.mul_(beta2).addcmul_(g, g, value=1.0 - beta2)
     bc1 = 1.0 - beta1 ** step
     bc2 = 1.0 - beta2 ** step
-    w.mul_(1.0 - lr * wd)
     denom = (v / bc2).sqrt_().add_(eps)
-    w.addcdiv_(m / bc1, denom, value=-lr)
+    if groups is None:
+        w.mul_(1.0 - lr * wd)
+        w.addcdiv_(m / bc1, denom, value=-lr)
+    else:
+        lr_e, decay = group_lr_decay(lr, groups, group_hyper, w.numel())
+        w.mul_(decay)
+        w.sub_(lr_e * (m / bc1) / denom)
 
 
 # Split fp32 master representation: fp32 bits == (hi_bf16_bits << 16) + lo_int16, hi = nearest bf16
@@ -583,11 +601,11 @@ def merge_fp32(hi, lo, w):
 
 
 def adamw_split(hi, lo, m, v, grad, clip, lr, beta1, beta2, eps, wd, step: int, hyper=None, ema=None,
-                ema_decay: float = 0.0):
-    """ema: optional (ema_hi, ema_lo), the model EMA in split form."""
+                ema_decay: float = 0.0, groups=None, group_hyper=None):
+    """ema: optional (ema_hi, ema_lo), the model EMA in split form.  groups / group_hyper: as in adamw_fp32."""
     w = torch.empty(hi.shape, dtype=torch.float32, device=hi.device)
     merge_fp32(hi, lo, w)
-    _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step)
+    _adamw_fp32(w, m, v, grad, clip, lr, beta1, beta2, eps, wd, step, groups, group_hyper)
     split_fp32(w, hi, lo)
     if ema is not None:
         e = torch.empty(hi.shape, dtype=torch.float32, device=hi.device)

@@ -27,6 +27,7 @@ from .config import ViTConfig
 from .data import build_datasets
 from .launch import Runtime
 from .parallel import FSDPViT, GraphedTrainStep, ShardedAdamW
+from .parallel.param_groups import format_summary
 from .utils import SmoothedValue, get_warmup_cosine_scheduler
 from .utils.checkpoint import load_ckpt, normalize_full_state_dict_keys, resize_pos_embed, save_ckpt
 
@@ -98,7 +99,9 @@ class TrainStep:
         want_graph = bool(getattr(cfg, "cuda_graph", False)) and device.type == "cuda"
         self.optimizer = ShardedAdamW(model, lr=cfg.lr, weight_decay=cfg.weight_decay,
                                       fuse_into_reduce_scatter=self.clip <= 0 and not want_graph and not model.has_ema,
-                                      model_ema_decay=float(cfg.model_ema_decay) if model.has_ema else None)
+                                      model_ema_decay=float(cfg.model_ema_decay) if model.has_ema else None,
+                                      filter_bias_and_norm=bool(getattr(cfg, "filter_bias_and_norm", False)),
+                                      layer_decay=getattr(cfg, "layer_decay", None))
         self.graph: Optional[GraphedTrainStep] = (
             GraphedTrainStep(model, self.optimizer, self.clip) if want_graph else None)
 
@@ -200,6 +203,9 @@ class Trainer:
             max_iteration=len(self.train_set) // cfg.batch_size * cfg.num_epochs)
         rt.rendezvous("loaded optimizer")
         say(f"\n=== optimizer ===\n{pprint.pformat(self.optimizer)}\n")
+        groups = self.optimizer.group_summary()
+        if groups is not None:
+            say(f"=== parameter groups ===\n{format_summary(groups)}\n")
 
         if getattr(cfg, "init_from_full_ckpt", ""):
             full = torch.load(cfg.init_from_full_ckpt, map_location="cpu", weights_only=False)
