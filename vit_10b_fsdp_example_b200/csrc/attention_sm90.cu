@@ -94,6 +94,8 @@ bool attention_supported(int N, int hd) {
     return shape_ok(N, hd) && (hd == 64 || hd == 128 || hd == 160 || tile_width(hd) <= 48);
 }
 
+bool attention_shape_ok(int N, int hd) { return shape_ok(N, hd); }
+
 void attention_fwd(const __nv_bfloat16* qkv, int64_t ld_qkv, __nv_bfloat16* out, float* lse, __nv_bfloat16* probs,
                    int64_t ldp, int B, int N, int H, int hd, cudaStream_t stream, float drop_p, uint64_t drop_key) {
     if (!shape_ok(N, hd)) throw std::runtime_error("attention_fwd: unsupported (N, head_dim)");
@@ -109,6 +111,7 @@ void attention_bwd(const __nv_bfloat16* qkv, int64_t ld_qkv, const __nv_bfloat16
                    const __nv_bfloat16* out, int64_t ld_o, const float* lse, float* delta, __nv_bfloat16* dqkv,
                    int B, int N, int H, int hd, cudaStream_t stream, float* colsum, float drop_p, uint64_t drop_key) {
     if (!shape_ok(N, hd)) throw std::runtime_error("attention_bwd: unsupported (N, head_dim)");
+    if (drop_p != 0.f) make_drop(drop_p, drop_key, "attention_bwd");  // a bad p throws before the delta kernel runs
     const int64_t warps = static_cast<int64_t>(B) * N * H;
     attn_delta_kernel<<<static_cast<unsigned>((warps + 7) / 8), 256, 0, stream>>>(dout, ld_do, out, ld_o, delta, B, N, H, hd);
     check_launch("attention delta launch");

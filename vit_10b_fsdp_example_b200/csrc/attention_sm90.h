@@ -11,6 +11,10 @@ namespace b200 {
 // routed); attention_fwd / attention_bwd throw on any other head dim.
 bool attention_supported(int N, int hd);
 
+// Whether the kernels take (N, hd) at all: even N >= 2 and a head dim listed above (attention_fwd / attention_bwd throw
+// otherwise).
+bool attention_shape_ok(int N, int hd);
+
 // qkv: packed [B*N, 3*H*hd] (row stride ld_qkv).  out: [B*N, H*hd].  lse: [B*H, N] fp32 or null.
 // probs: normalised softmax [B*H, N, ldp] bf16 or null (only written when the un-fused backward needs it).
 // drop_p > 0: attention dropout with the mask the dropout kernel (dropout.cuh) draws for key drop_key over the

@@ -110,13 +110,61 @@ void softmax_bwd(Tensor dp, Tensor p, int64_t rows, int64_t n, int64_t ld, doubl
 
 bool attention_supported(int64_t N, int64_t hd) { return b200::attention_supported((int)N, (int)hd); }
 
+// Argument checks of the attention entry points, all made before anything is launched.  The kernels read q / k / v
+// and dO through TMA (16-byte aligned base, row stride a multiple of 8 elements), read O as bf16 pairs in the delta
+// kernel, store O, dqkv and the probabilities as bf16 pairs (4-byte aligned, even row stride) and read lse / delta as
+// float2 in the dK / dV role (8-byte aligned).
+inline bool aligned(const Tensor& t, int64_t bytes) { return reinterpret_cast<uintptr_t>(t.data_ptr()) % bytes == 0; }
+
+// A [rows, cols] bf16 matrix with unit column stride on qkv's device, row stride >= cols and a multiple of ld_mult,
+// base aligned to `align` bytes.
+void check_matrix(const char* what, const char* name, const Tensor& t, const Tensor& like, int64_t rows, int64_t cols,
+                  int64_t ld_mult, int64_t align) {
+    TORCH_CHECK(t.is_cuda() && t.device() == like.device() && t.scalar_type() == at::kBFloat16, what, ": ", name,
+                " must be a bf16 tensor on ", like.device());
+    TORCH_CHECK(t.dim() == 2 && t.size(0) == rows && t.size(1) == cols, what, ": ", name, " must be [", rows, ", ",
+                cols, "], got ", t.sizes());
+    TORCH_CHECK(t.stride(1) == 1 && t.stride(0) >= cols && t.stride(0) % ld_mult == 0, what, ": ", name,
+                " needs unit column stride and a row stride >= ", cols, " that is a multiple of ", ld_mult, ", got ",
+                t.strides());
+    TORCH_CHECK(aligned(t, align), what, ": ", name, " must be ", align, "-byte aligned");
+}
+
+// A contiguous fp32 vector of n elements on qkv's device, base aligned to `align` bytes.
+void check_f32(const char* what, const char* name, const Tensor& t, const Tensor& like, int64_t n, int64_t align) {
+    TORCH_CHECK(t.is_cuda() && t.device() == like.device() && t.scalar_type() == at::kFloat, what, ": ", name,
+                " must be an fp32 tensor on ", like.device());
+    TORCH_CHECK(t.is_contiguous() && t.numel() == n, what, ": ", name, " must be contiguous with ", n,
+                " elements, got ", t.sizes());
+    TORCH_CHECK(aligned(t, align), what, ": ", name, " must be ", align, "-byte aligned");
+}
+
+void check_attention_dims(const char* what, int64_t B, int64_t N, int64_t H, int64_t hd, double drop_p) {
+    TORCH_CHECK(B >= 1 && H >= 1, what, ": need B >= 1 and H >= 1");
+    TORCH_CHECK(b200::attention_shape_ok((int)N, (int)hd), what, ": unsupported (N, head_dim) = (", N, ", ", hd, ")");
+    TORCH_CHECK(drop_p == 0.0 || (drop_p > 0.0 && drop_p < 1.0), what, ": dropout p must be 0 or in (0, 1)");
+}
+
 // drop_p > 0: attention dropout with the mask `dropout` draws for drop_key over [B*H, N, pad8(N)] probabilities.
 void attention_fwd(Tensor qkv, Tensor out, OptT lse, OptT probs, int64_t B, int64_t N, int64_t H, int64_t hd,
                    double drop_p, int64_t drop_key) {
     c10::cuda::CUDAGuard guard(qkv.device());
-    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && out.is_contiguous(), "attention_fwd: bad layouts");
-    TORCH_CHECK(!lse.has_value() || (lse->is_contiguous() && lse->numel() == B * H * N), "attention_fwd: bad lse");
+    const char* what = "attention_fwd";
+    check_attention_dims(what, B, N, H, hd, drop_p);
+    const int64_t D = H * hd;
+    check_matrix(what, "qkv", qkv, qkv, B * N, 3 * D, 8, 16);
+    check_matrix(what, "out", out, qkv, B * N, D, 2, 4);
+    TORCH_CHECK(out.is_contiguous(), "attention_fwd: out must be contiguous (the kernels store it with row stride D)");
+    if (lse.has_value()) check_f32(what, "lse", *lse, qkv, B * H * N, 4);
     TORCH_CHECK(drop_p == 0.0 || !probs.has_value(), "attention_fwd: no probability output with dropout");
+    if (probs.has_value()) {
+        const Tensor& p = *probs;
+        TORCH_CHECK(p.is_cuda() && p.device() == qkv.device() && p.scalar_type() == at::kBFloat16,
+                    "attention_fwd: probs must be a bf16 tensor on ", qkv.device());
+        TORCH_CHECK(p.dim() == 3 && p.size(0) == B * H && p.size(1) == N && p.size(2) >= N && p.size(2) % 2 == 0,
+                    "attention_fwd: probs must be [B*H, N, ldp] with an even ldp >= N, got ", p.sizes());
+        TORCH_CHECK(p.is_contiguous() && aligned(p, 4), "attention_fwd: probs must be contiguous and 4-byte aligned");
+    }
     b200::attention_fwd(bf16_ptr(qkv), qkv.stride(0), bf16_mut(out), lse.has_value() ? f32_ptr(*lse) : nullptr,
                         probs.has_value() ? bf16_mut(*probs) : nullptr, probs.has_value() ? probs->size(2) : 0, (int)B,
                         (int)N, (int)H, (int)hd, cur_stream(), (float)drop_p, (uint64_t)drop_key);
@@ -125,11 +173,17 @@ void attention_fwd(Tensor qkv, Tensor out, OptT lse, OptT probs, int64_t B, int6
 void attention_bwd(Tensor qkv, Tensor dout, Tensor out, Tensor lse, Tensor delta, Tensor dqkv, OptT colsum, int64_t B,
                    int64_t N, int64_t H, int64_t hd, double drop_p, int64_t drop_key) {
     c10::cuda::CUDAGuard guard(qkv.device());
-    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && dout.stride(1) == 1 && out.stride(1) == 1 &&
-                    dqkv.is_contiguous() && lse.is_contiguous() && delta.is_contiguous(),
-                "attention_bwd: bad layouts");
-    TORCH_CHECK(lse.numel() == B * H * N && delta.numel() == B * H * N && dqkv.size(1) == 3 * H * hd,
-                "attention_bwd: bad shapes");
+    const char* what = "attention_bwd";
+    check_attention_dims(what, B, N, H, hd, drop_p);
+    const int64_t D = H * hd;
+    check_matrix(what, "qkv", qkv, qkv, B * N, 3 * D, 8, 16);
+    check_matrix(what, "dout", dout, qkv, B * N, D, 8, 16);
+    check_matrix(what, "out", out, qkv, B * N, D, 2, 4);
+    check_f32(what, "lse", lse, qkv, B * H * N, 8);
+    check_f32(what, "delta", delta, qkv, B * H * N, 8);
+    check_matrix(what, "dqkv", dqkv, qkv, B * N, 3 * D, 2, 4);
+    TORCH_CHECK(dqkv.is_contiguous(), "attention_bwd: dqkv must be contiguous (the kernels store it with row stride 3 D)");
+    if (colsum.has_value()) check_f32(what, "colsum", *colsum, qkv, 3 * D, 4);
     b200::attention_bwd(bf16_ptr(qkv), qkv.stride(0), bf16_ptr(dout), dout.stride(0), bf16_ptr(out), out.stride(0),
                         f32_ptr(lse), f32_ptr(delta), bf16_mut(dqkv), (int)B, (int)N, (int)H, (int)hd, cur_stream(),
                         colsum.has_value() ? f32_ptr(*colsum) : nullptr, (float)drop_p, (uint64_t)drop_key);

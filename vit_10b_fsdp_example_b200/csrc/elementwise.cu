@@ -1453,12 +1453,12 @@ static void check_softmax_args(const void* a, const void* b, int n, int64_t ld) 
 
 void softmax_fwd(__nv_bfloat16* s, int64_t rows, int n, int64_t ld, float scale, cudaStream_t stream) {
     check_softmax_args(s, s, n, ld);
+    if (rows == 0) return;
     const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
     if (softmax_pairs(n)) {
         const int pairs_per_lane = (n / 2 + 31) / 32;
         SM_DISPATCH(softmax_fwd_kernel, s, rows, n, ld, scale);
     } else {
-        if (rows == 0) return;
         const int vecs_per_lane = ((n + 7) / 8 + 31) / 32;
         SM_VEC_DISPATCH(softmax_fwd_vec_kernel, softmax_fwd_long_kernel, s, rows, n, ld, scale);
     }
@@ -1468,12 +1468,12 @@ void softmax_fwd(__nv_bfloat16* s, int64_t rows, int n, int64_t ld, float scale,
 void softmax_bwd(__nv_bfloat16* dp, const __nv_bfloat16* p, int64_t rows, int n, int64_t ld, float scale,
                  cudaStream_t stream) {
     check_softmax_args(dp, p, n, ld);
+    if (rows == 0) return;
     const unsigned grid = static_cast<unsigned>((rows + 7) / 8);
     if (softmax_pairs(n)) {
         const int pairs_per_lane = (n / 2 + 31) / 32;
         SM_DISPATCH(softmax_bwd_kernel, dp, p, rows, n, ld, scale);
     } else {
-        if (rows == 0) return;
         const int vecs_per_lane = ((n + 7) / 8 + 31) / 32;
         SM_VEC_DISPATCH(softmax_bwd_vec_kernel, softmax_bwd_long_kernel, dp, p, rows, n, ld, scale);
     }
