@@ -37,6 +37,20 @@ def sass_hash(obj, name):
     return hashlib.sha256("\n".join(ins).encode()).hexdigest()
 
 
+def ptxas_usage(log):
+    """{symbol key: [registers, spill store bytes, spill load bytes]} from `-Xptxas -v` output."""
+    lines = log.splitlines()
+    usage = {}
+    for i, ln in enumerate(lines):
+        if "Compiling entry function" in ln:
+            spill = next(x for x in lines[i + 1:] if "spill stores" in x)
+            regs = next(x for x in lines[i + 1:] if re.search(r"Used \d+ registers", x))
+            st, ld = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", spill).groups()
+            usage[sass_symbol_key(ln.split("'")[1])] = [int(re.search(r"Used (\d+) registers", regs).group(1)), int(st),
+                                                        int(ld)]
+    return usage
+
+
 def free_port():
     with socket.socket(socket.AF_INET, socket.SOCK_STREAM) as s:
         s.bind(("127.0.0.1", 0))

@@ -21,6 +21,7 @@
 
 #include "dropout.cuh"
 #include "elementwise.h"
+#include "epilogue_math.cuh"
 #include "im2col_pixel.cuh"
 #include "ptx.cuh"
 
@@ -431,17 +432,6 @@ __global__ void __launch_bounds__(kLnThreads) ln_bwd_small_kernel(const __nv_bfl
 // MMA time of a tile, so the fused epilogue would run the tensor cores at half speed; the op layer then uses the
 // plain GEMM plus these memory-bound kernels (for ViT-10B, K = 5120, the activations stay fused in the epilogue).
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float erf_poly(float z, float& e) {
-    const float az = fabsf(z);
-    const float t = __frcp_rn(fmaf(0.3275911f, az, 1.0f));
-    e = __expf(-az * az);
-    float poly = fmaf(1.061405429f, t, -1.453152027f);
-    poly = fmaf(poly, t, 1.421413741f);
-    poly = fmaf(poly, t, -0.284496736f);
-    poly = fmaf(poly, t, 0.254829592f);
-    return copysignf(1.0f - poly * t * e, z);
-}
-
 __global__ void __launch_bounds__(256) gelu_fwd_kernel(const __nv_bfloat16* __restrict__ u, __nv_bfloat16* __restrict__ g,
                                                        int64_t nvec) {
     for (int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < nvec;
@@ -478,15 +468,9 @@ __global__ void __launch_bounds__(256) dgelu_mul_kernel(const __nv_bfloat16* __r
 // ------------------------------------------------------------------------------------------------
 // Stand-alone SwiGLU (timm SwiGLUPacked): u = [gate | value] [M, 2H'], g = silu(gate) * value [M, H'].  The short-K
 // counterparts of the GEMM's SwiGLU / dSwiGLU epilogues, and the re-materialisation of g in backward.  One thread owns 8
-// adjacent columns of one row (16-byte vectors of the gate, the value and the output); sigmoid is rcp.approx(1 + exp(-x)),
-// exactly as in the GEMM epilogue, so the fused and unfused routes compute the same function.
+// adjacent columns of one row (16-byte vectors of the gate, the value and the output); sigmoid is the GEMM epilogue's
+// sigmoid_approx (epilogue_math.cuh), so the fused and unfused routes compute the same function.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float swiglu_sigmoid(float x) {
-    float r;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + __expf(-x)));
-    return r;
-}
-
 __global__ void __launch_bounds__(256) swiglu_fwd_kernel(const __nv_bfloat16* __restrict__ u,
                                                          __nv_bfloat16* __restrict__ g, int64_t M, int hvec) {
     // rows over grid.y, 16-byte column vectors over grid.x: no 64-bit division (it would be a subroutine call)
@@ -498,7 +482,7 @@ __global__ void __launch_bounds__(256) swiglu_fwd_kernel(const __nv_bfloat16* __
         unpack8(ur[cv], a);
         unpack8(ur[hvec + cv], b);
 #pragma unroll
-        for (int q = 0; q < 8; ++q) b[q] *= a[q] * swiglu_sigmoid(a[q]);
+        for (int q = 0; q < 8; ++q) b[q] *= a[q] * sigmoid_approx(a[q]);
         reinterpret_cast<uint4*>(g)[i] = pack8(b);
     }
 }
@@ -517,7 +501,7 @@ __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const __nv_bfloat16* __
         unpack8(reinterpret_cast<const uint4*>(dg)[i], d);
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
-            const float s = swiglu_sigmoid(a[q]);
+            const float s = sigmoid_approx(a[q]);
             const float dq = d[q];
             d[q] = dq * b[q] * (s * fmaf(a[q], 1.0f - s, 1.0f));  // du_gate = dg * b * silu'(a)
             b[q] = dq * (a[q] * s);                               // du_val  = dg * silu(a)

@@ -30,6 +30,7 @@
 #include <algorithm>
 #include <unordered_map>
 
+#include "epilogue_math.cuh"
 #include "gemm_sm90.h"
 #include "ptx.cuh"
 #include "wgmma.cuh"
@@ -78,39 +79,33 @@ __device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* ptr) {
 }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
-// erf via Abramowitz-Stegun 7.1.26 (|err| < 1.5e-7, far below bf16 resolution): 1 rcp + 1 exp + 6 FMA.
-// e = exp(-z^2) is returned too: for z = x/sqrt(2) it is exactly the Gaussian factor gelu'(x) needs.
-__device__ __forceinline__ float rcp_approx(float x) {
-    float r;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-    return r;
+// Byte offset of column `col` of 16-byte chunk `chunk` in row `row` of a 64 x 64 bf16 staging buffer: the chunk is
+// XOR-swizzled with the row, as the SWIZZLE_128B TMA store expects.
+template <typename I>
+__device__ __forceinline__ I swizzled_offset(I row, I chunk, I col) {
+    return row * 128 + ((chunk ^ (row & 7)) * 16) + col * 2;
 }
-__device__ __forceinline__ float erf_as(float z, float& e) {
-    const float az = fabsf(z);
-    // rcp.approx (relative error <= 2^-23, below the 1.5e-7 of the formula) rather than __frcp_rn: the correctly
-    // rounded reciprocal calls a slow-path subroutine, and the GEMM kernel must stay free of calls (see its body).
-    // The argument is >= 1, never in that slow range.
-    const float t = rcp_approx(fmaf(0.3275911f, az, 1.0f));
-    e = __expf(-az * az);
-    float poly = fmaf(1.061405429f, t, -1.453152027f);
-    poly = fmaf(poly, t, 1.421413741f);
-    poly = fmaf(poly, t, -0.284496736f);
-    poly = fmaf(poly, t, 0.254829592f);
-    const float y = 1.0f - poly * t * e;
-    return copysignf(y, z);
+
+// One accumulator quad of chunk j to a staging buffer: v[0..1] to row wrow, v[2..3] to row wrow + 8 (same swizzle).
+__device__ __forceinline__ void stage_pair(uint8_t* buf, uint32_t wrow, int j, uint32_t cpair, const float (&v)[4]) {
+    const uint32_t off0 = swizzled_offset<uint32_t>(wrow, j, cpair);
+    st_shared_b32(smem_u32(buf) + off0, pack_bf16x2(v[0], v[1]));
+    st_shared_b32(smem_u32(buf) + off0 + 8 * 128, pack_bf16x2(v[2], v[3]));
 }
-__device__ __forceinline__ float gelu_erf(float x) {
-    float e;
-    return 0.5f * x * (1.0f + erf_as(x * 0.70710678118654752f, e));
+
+// Bias gradient: thread etid sums column etid % 64 of the staged (bf16-rounded) chunk `buf` over rows [0, 32) or [32, 64).
+__device__ __forceinline__ float column_sum(const uint8_t* buf, uint32_t etid) {
+    const int ccol = etid & 63;       // column within the chunk
+    const int rhalf = etid >> 6;      // 0/1 -> rows [0,32) / [32,64)
+    const int jj = ccol >> 3, within = ccol & 7;
+    float s = 0.f;
+#pragma unroll 8
+    for (int r = 0; r < 32; ++r) {
+        const int rr = rhalf * 32 + r;
+        s += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(buf + swizzled_offset<int>(rr, jj, within)));
+    }
+    return s;
 }
-__device__ __forceinline__ float dgelu_erf(float x) {
-    float e;
-    const float cdf = 0.5f * (1.0f + erf_as(x * 0.70710678118654752f, e));
-    return fmaf(x * 0.3989422804014327f, e, cdf);  // cdf + x * pdf,  pdf = exp(-x^2/2)/sqrt(2 pi)
-}
-// sigmoid(x) = 1 / (1 + exp(-x)) with ex2.approx and rcp.approx: no call.  exp(-x) overflows to inf for x < -88 and the
-// reciprocal of inf is 0, so silu(x) = x * sigmoid(x) and silu'(x) = s (1 + x (1 - s)) go to -0 / 0 there, as they should.
-__device__ __forceinline__ float sigmoid_approx(float x) { return rcp_approx(1.0f + __expf(-x)); }
 
 // kClusterM = 2: CTAs run in (2, 1, 1) clusters.  The two CTAs of a cluster own m-tiles 2 mp and 2 mp + 1 of the same
 // (batch, n-tile), so they need the same B tile: each producer loads its own A tile and one half of B, multicast to
@@ -426,11 +421,8 @@ __device__ __forceinline__ void gemm_bf16_sm90_body(const CUtensorMap& tmap_a, c
                         for (int j = 0; j < 8; ++j) {
                             float a[4], v[4];
                             gate_value(c, j, a, v);
-                            const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
-                            st_shared_b32(smem_u32(grp_buf) + off0, pack_bf16x2(a[0], a[1]));
-                            st_shared_b32(smem_u32(grp_buf) + off0 + 8 * 128, pack_bf16x2(a[2], a[3]));
-                            st_shared_b32(smem_u32(grp_buf + kCdBufBytes) + off0, pack_bf16x2(v[0], v[1]));
-                            st_shared_b32(smem_u32(grp_buf + kCdBufBytes) + off0 + 8 * 128, pack_bf16x2(v[2], v[3]));
+                            stage_pair(grp_buf, wrow, j, cpair, a);
+                            stage_pair(grp_buf + kCdBufBytes, wrow, j, cpair, v);
                         }
                         fence_proxy_async_smem();
                         named_bar_sync(bar_id, kEpiThreads);
@@ -451,9 +443,7 @@ __device__ __forceinline__ void gemm_bf16_sm90_body(const CUtensorMap& tmap_a, c
                         gate_value(c, j, a, v);
 #pragma unroll
                         for (int q = 0; q < 4; ++q) v[q] *= a[q] * sigmoid_approx(a[q]);
-                        const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
-                        st_shared_b32(smem_u32(buf0) + off0, pack_bf16x2(v[0], v[1]));
-                        st_shared_b32(smem_u32(buf0) + off0 + 8 * 128, pack_bf16x2(v[2], v[3]));
+                        stage_pair(buf0, wrow, j, cpair, v);
                     }
                     fence_proxy_async_smem();
                     named_bar_sync(bar_id, kEpiThreads);
@@ -502,11 +492,8 @@ __device__ __forceinline__ void gemm_bf16_sm90_body(const CUtensorMap& tmap_a, c
                             dv[q] = ok ? dh * (a * sg) : 0.f;  // zeros keep the column sums clean
                             dg[q] = ok ? dh * b * (sg * fmaf(a, 1.0f - sg, 1.0f)) : 0.f;
                         }
-                        const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
-                        st_shared_b32(smem_u32(buf0) + off0, pack_bf16x2(dg[0], dg[1]));
-                        st_shared_b32(smem_u32(buf0) + off0 + 8 * 128, pack_bf16x2(dg[2], dg[3]));
-                        st_shared_b32(smem_u32(buf1) + off0, pack_bf16x2(dv[0], dv[1]));
-                        st_shared_b32(smem_u32(buf1) + off0 + 8 * 128, pack_bf16x2(dv[2], dv[3]));
+                        stage_pair(buf0, wrow, j, cpair, dg);
+                        stage_pair(buf1, wrow, j, cpair, dv);
                     }
                     fence_proxy_async_smem();
                     named_bar_sync(bar_id, kEpiThreads);
@@ -524,7 +511,7 @@ __device__ __forceinline__ void gemm_bf16_sm90_body(const CUtensorMap& tmap_a, c
 #pragma unroll 8
                         for (int r = 0; r < 32; ++r) {
                             const int rr = rhalf * 32 + r;
-                            const int off = rr * 128 + ((jj ^ (rr & 7)) * 16) + within * 2;
+                            const int off = swizzled_offset<int>(rr, jj, within);
                             s0 += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(buf0 + off));
                             s1 += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(buf1 + off));
                         }
@@ -581,7 +568,7 @@ __device__ __forceinline__ void gemm_bf16_sm90_body(const CUtensorMap& tmap_a, c
                             v[0] += bf16_lo(bw), v[1] += bf16_hi(bw), v[2] += bf16_lo(bw), v[3] += bf16_hi(bw);
                         }
                         // 16-byte chunk j of a 128-byte row, XOR-swizzled with the row like the TMA store expects
-                        const uint32_t off0 = wrow * 128 + ((j ^ (wrow & 7)) * 16) + cpair * 2;
+                        const uint32_t off0 = swizzled_offset<uint32_t>(wrow, j, cpair);
                         const uint32_t off1 = off0 + 8 * 128;  // row + 8 has the same (row & 7)
                         if (e.has_aux_out) {
                             st_shared_b32(smem_u32(buf1) + off0, pack_bf16x2(v[0], v[1]));
@@ -620,16 +607,8 @@ __device__ __forceinline__ void gemm_bf16_sm90_body(const CUtensorMap& tmap_a, c
                     }
                     if (e.colsum != nullptr) {
                         // Bias gradient: column sums of the (bf16-rounded) output tile, fp32 atomics.
-                        const int ccol = etid & 63;       // column within the chunk
-                        const int rhalf = etid >> 6;      // 0/1 -> rows [0,32) / [32,64)
-                        const int jj = ccol >> 3, within = ccol & 7;
-                        float s = 0.f;
-    #pragma unroll 8
-                        for (int r = 0; r < 32; ++r) {
-                            const int rr = rhalf * 32 + r;
-                            const uint8_t* ptr = buf0 + rr * 128 + ((jj ^ (rr & 7)) * 16) + within * 2;
-                            s += __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(ptr));
-                        }
+                        const int ccol = etid & 63;
+                        const float s = column_sum(buf0, etid);
                         if (ncol0 + ccol < p.N)
                             atomicAdd(e.colsum + static_cast<int64_t>(bi) * e.colsum_bi_stride + ncol0 + ccol, s);
                     }
@@ -853,6 +832,25 @@ void launch(const GemmOperand& A, const GemmOperand& B, const GemmOperand& D, co
     check(cudaGetLastError(), "gemm launch failed");
 }
 
+// The instantiation for a run-time tile width and cluster size: 256-wide tiles with a 4-stage ring, 128-wide ones with
+// 6 stages, each in 1-CTA or 2-CTA clusters.  Returns false when there is none for `block_n`.
+template <int kMajorA, int kMajorB, bool kRowScale = false, int kGlu = 0>
+bool launch_for(int block_n, int cluster, const GemmOperand& A, const GemmOperand& B, const GemmOperand& D,
+                const GemmOperand* aux, int M, int N, int K, const GemmEpilogue& epi, int max_ctas,
+                cudaStream_t stream, const GemmAgFuse* ag) {
+    if (block_n == 256 && cluster == 2)
+        launch<kMajorA, kMajorB, 256, 4, 2, kRowScale, kGlu>(A, B, D, aux, M, N, K, epi, max_ctas, stream, ag);
+    else if (block_n == 256)
+        launch<kMajorA, kMajorB, 256, 4, 1, kRowScale, kGlu>(A, B, D, aux, M, N, K, epi, max_ctas, stream, ag);
+    else if (block_n == 128 && cluster == 2)
+        launch<kMajorA, kMajorB, 128, 6, 2, kRowScale, kGlu>(A, B, D, aux, M, N, K, epi, max_ctas, stream, ag);
+    else if (block_n == 128)
+        launch<kMajorA, kMajorB, 128, 6, 1, kRowScale, kGlu>(A, B, D, aux, M, N, K, epi, max_ctas, stream, ag);
+    else
+        return false;
+    return true;
+}
+
 // SwiGLU epilogues: the checks that keep them within what the kernel implements, each named in its message.
 void gemm_glu(const GemmOperand& A, int major_a, const GemmOperand& B, int major_b, const GemmOperand& D,
               const GemmOperand* aux_out, int M, int N, int K, const GemmEpilogue& epi, int block_n, int cluster,
@@ -879,14 +877,10 @@ void gemm_glu(const GemmOperand& A, int major_a, const GemmOperand& B, int major
     if (block_n == 0) block_n = 256;
     if (block_n != 128 && block_n != 256) throw std::runtime_error("gemm: SwiGLU block_n must be 128 or 256");
     if (cluster == 0 || max_ctas == 1) cluster = 1;
-#define B200_GLU(MB, BN, ST, ACT)                                                                            \
-    cluster == 2 ? launch<0, MB, BN, ST, 2, false, ACT>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag) \
-                 : launch<0, MB, BN, ST, 1, false, ACT>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag)
     if (fwd)
-        block_n == 256 ? B200_GLU(0, 256, 4, kActSwiglu) : B200_GLU(0, 128, 6, kActSwiglu);
+        launch_for<0, 0, false, kActSwiglu>(block_n, cluster, A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
     else
-        block_n == 256 ? B200_GLU(1, 256, 4, kActDSwiglu) : B200_GLU(1, 128, 6, kActDSwiglu);
-#undef B200_GLU
+        launch_for<0, 1, false, kActDSwiglu>(block_n, cluster, A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
 }
 
 }  // namespace
@@ -919,34 +913,20 @@ void gemm_bf16(const GemmOperand& A, int major_a, const GemmOperand& B, int majo
             D.nb_inner * D.nb_outer > 1)
             throw std::runtime_error("gemm: row_scale only with no activation, no aux output, no column sums, unbatched");
         if (major_a != 0 || major_b != 0) throw std::runtime_error("gemm: row_scale needs K-major A and B");
-        if (block_n == 256)
-            cluster == 2 ? launch<0, 0, 256, 4, 2, true>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag)
-                         : launch<0, 0, 256, 4, 1, true>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
-        else if (block_n == 128)
-            cluster == 2 ? launch<0, 0, 128, 6, 2, true>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag)
-                         : launch<0, 0, 128, 6, 1, true>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
-        else
+        if (!launch_for<0, 0, true>(block_n, cluster, A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag))
             throw std::runtime_error("gemm: unsupported block_n");
         return;
     }
-#define B200_DISPATCH(MA, MB, BN, ST)                                                             \
-    if (major_a == MA && major_b == MB && block_n == BN) {                                        \
-        if (cluster == 2)                                                                         \
-            launch<MA, MB, BN, ST, 2>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);      \
-        else                                                                                      \
-            launch<MA, MB, BN, ST, 1>(A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);      \
-        return;                                                                                   \
-    }
-    B200_DISPATCH(0, 0, 256, 4)
-    B200_DISPATCH(0, 1, 256, 4)
-    B200_DISPATCH(1, 1, 256, 4)
-    B200_DISPATCH(1, 0, 256, 4)
-    B200_DISPATCH(0, 0, 128, 6)
-    B200_DISPATCH(0, 1, 128, 6)
-    B200_DISPATCH(1, 1, 128, 6)
-    B200_DISPATCH(1, 0, 128, 6)
-#undef B200_DISPATCH
-    throw std::runtime_error("gemm: unsupported (major_a, major_b, block_n) combination");
+    bool launched = false;
+    if (major_a == 0 && major_b == 0)
+        launched = launch_for<0, 0>(block_n, cluster, A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
+    else if (major_a == 0 && major_b == 1)
+        launched = launch_for<0, 1>(block_n, cluster, A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
+    else if (major_a == 1 && major_b == 1)
+        launched = launch_for<1, 1>(block_n, cluster, A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
+    else if (major_a == 1 && major_b == 0)
+        launched = launch_for<1, 0>(block_n, cluster, A, B, D, aux_out, M, N, K, epi, max_ctas, stream, ag);
+    if (!launched) throw std::runtime_error("gemm: unsupported (major_a, major_b, block_n) combination");
 }
 
 }  // namespace b200
