@@ -22,7 +22,7 @@ SO_PATH = os.path.join(PKG_DIR, "_C.so")
 
 CU_SOURCES = ["gemm_sm90.cu", "elementwise.cu", "comm.cu", "attention_sm90.cu", "attention_drop_sm90.cu",
               "layernorm_stream.cu", "qk_norm.cu", "layer_scale.cu", "prefix_tokens.cu",
-              "patch_drop.cu"]
+              "patch_drop.cu", "rope.cu"]
 CPP_SOURCES = ["bindings.cpp"]
 
 NVCC_FLAGS = [

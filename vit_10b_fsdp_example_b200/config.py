@@ -109,6 +109,19 @@ def build_arg_parser() -> argparse.ArgumentParser:
                         help="patch dropout (timm PatchDropout; Liu et al. 2022, FLIP): in training every image keeps "
                              "a random max(1, int(N * (1 - rate))) of its N patch tokens (the class / register tokens "
                              "always), so every block runs on fewer tokens; evaluation keeps all; 0 = off")
+    # ---- rotary position embedding (EVA-02: timm Eva(use_rot_pos_emb=True), RotaryEmbeddingCat) ----
+    parser.add_argument("--rope", action="store_true",
+                        help="2-D axial rotary position embedding (EVA-02, timm RotaryEmbeddingCat) on the queries and "
+                             "keys of every block, after --qk_norm, on top of the learned pos_embed: of the hd / 2 "
+                             "interleaved pairs of a head, the first hd / 4 turn with the patch row, the rest with the "
+                             "patch column; class and register tokens are not rotated; needs head_dim % 4 == 0")
+    parser.add_argument("--rope_theta", type=_rope_theta, default=ROPE_THETA,
+                        help="RoPE base theta: pair j of a half turns with frequency theta ** (-j / (head_dim / 4)); "
+                             "needs --rope")
+    parser.add_argument("--rope_ref_grid", type=_rope_ref_grid, default=0,
+                        help="RoPE reference grid g_ref (timm ref_feat_shape): positions are scaled by g_ref / grid, "
+                             "so a fine-tune at a higher resolution keeps the pre-training angles when g_ref is the "
+                             "pre-training grid; 0 = the run's own grid; needs --rope")
     # ---- model EMA (timm ModelEmaV2; DeiT --model-ema) ----
     parser.add_argument("--model_ema", action="store_true",
                         help="keep an exponential moving average of the weights (timm ModelEmaV2, DeiT --model-ema), "
@@ -147,6 +160,35 @@ def check_prefix_flags(args) -> None:
         flag = "--reg_tokens" if args.reg_tokens else "--no_embed_class"
         raise ValueError(f"{flag} needs --class_token (register tokens and an un-embedded prefix exist only next to a "
                          f"class token; mean pooling has no prefix tokens)")
+
+
+ROPE_THETA = 10000.0  # timm RotaryEmbeddingCat temperature
+
+
+def check_rope(cfg) -> None:
+    """--rope_theta / --rope_ref_grid only mean something with --rope, and the rotation splits every head into two
+    halves of interleaved pairs, so --rope needs head_dim % 4 == 0."""
+    rope = getattr(cfg, "rope", False)
+    if not rope and (getattr(cfg, "rope_theta", ROPE_THETA) != ROPE_THETA or getattr(cfg, "rope_ref_grid", 0)):
+        flag = "--rope_theta" if getattr(cfg, "rope_theta", ROPE_THETA) != ROPE_THETA else "--rope_ref_grid"
+        raise ValueError(f"{flag} needs --rope (it sets the rotary position embedding, which is off)")
+    if rope and cfg.embed_dim % cfg.num_heads == 0 and (cfg.embed_dim // cfg.num_heads) % 4 != 0:
+        raise ValueError(f"--rope needs head_dim % 4 == 0 (hd / 4 frequency pairs for the patch row and as many for the "
+                         f"column), got head_dim = {cfg.embed_dim // cfg.num_heads}")
+
+
+def _rope_theta(s: str) -> float:
+    v = float(s)
+    if not (v > 0.0 and v != float("inf")):
+        raise argparse.ArgumentTypeError(f"--rope_theta must be a finite number > 0, got {s}")
+    return v
+
+
+def _rope_ref_grid(s: str) -> int:
+    v = int(s)
+    if v < 0:
+        raise argparse.ArgumentTypeError(f"--rope_ref_grid must be an integer >= 0, got {s}")
+    return v
 
 
 def _drop_path_rate(s: str) -> float:
@@ -215,6 +257,7 @@ def parse_args(argv=None) -> argparse.Namespace:
     try:
         check_prefix_flags(args)
         check_swiglu(args)
+        check_rope(args)
     except ValueError as e:
         parser.error(str(e))
     return args
@@ -245,6 +288,9 @@ class ViTConfig:
     no_embed_class: bool = False  # pos_embed covers the patches only (timm no_embed_class=True; needs class_token)
     swiglu: bool = False  # SwiGLU MLP (timm SwiGLUPacked): fc1 -> [gate | value] of width hidden_dim, fc2 reads half of it
     patch_drop_rate: float = 0.0  # patch dropout in training (timm PatchDropout, ordered); 0 = off
+    rope: bool = False  # 2-D axial rotary position embedding on q and k (EVA-02, timm RotaryEmbeddingCat)
+    rope_theta: float = ROPE_THETA  # RoPE base
+    rope_ref_grid: int = 0  # RoPE reference grid (timm ref_feat_shape); 0 = the run's grid
 
     def __post_init__(self):
         if not 0.0 <= self.drop_path_rate < 1.0:
@@ -264,8 +310,13 @@ class ViTConfig:
             raise ValueError(f"reg_tokens must be an integer >= 0, got {self.reg_tokens}")
         if not 0.0 <= self.patch_drop_rate < 1.0:
             raise ValueError(f"patch_drop_rate must be in [0, 1), got {self.patch_drop_rate}")
+        if not (self.rope_theta > 0.0 and self.rope_theta != float("inf")):
+            raise ValueError(f"rope_theta must be a finite number > 0, got {self.rope_theta}")
+        if not (isinstance(self.rope_ref_grid, int) and self.rope_ref_grid >= 0):
+            raise ValueError(f"rope_ref_grid must be an integer >= 0, got {self.rope_ref_grid}")
         check_prefix_flags(self)
         check_swiglu(self)
+        check_rope(self)
 
     @property
     def mixing(self) -> bool:
@@ -283,7 +334,9 @@ class ViTConfig:
                    smoothing=getattr(cfg, "smoothing", 0.0), qk_norm=getattr(cfg, "qk_norm", False),
                    init_values=getattr(cfg, "init_values", 0.0), class_token=getattr(cfg, "class_token", False),
                    reg_tokens=getattr(cfg, "reg_tokens", 0), no_embed_class=getattr(cfg, "no_embed_class", False),
-                   swiglu=getattr(cfg, "swiglu", False), patch_drop_rate=getattr(cfg, "patch_drop_rate", 0.0))
+                   swiglu=getattr(cfg, "swiglu", False), patch_drop_rate=getattr(cfg, "patch_drop_rate", 0.0),
+                   rope=getattr(cfg, "rope", False), rope_theta=getattr(cfg, "rope_theta", ROPE_THETA),
+                   rope_ref_grid=getattr(cfg, "rope_ref_grid", 0))
 
     @property
     def grid(self) -> int:

@@ -4,6 +4,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
+#include <climits>
 #include <cmath>
 #include <optional>
 #include <vector>
@@ -15,6 +16,7 @@
 #include "layer_scale.h"
 #include "patch_drop.h"
 #include "prefix_tokens.h"
+#include "rope.h"
 
 namespace {
 
@@ -278,36 +280,109 @@ void swiglu_bwd(Tensor dg, Tensor u, Tensor du) {
 }
 
 // qkv / out: [T, >= 3 H hd] row-major bf16 (out may be qkv: in place); mean / rstd: fp32 [T * 2 * H].
+void check_qk_norm_fwd(const char* what, const Tensor& qkv, const Tensor& wq, const Tensor& bq, const Tensor& wk,
+                       const Tensor& bk, const Tensor& out, const Tensor& mean, const Tensor& rstd, int64_t H,
+                       int64_t hd) {
+    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && out.dim() == 2 && out.stride(1) == 1 &&
+                    out.size(0) == qkv.size(0), what, ": qkv and out must be row-major [T, 3D] matrices");
+    const int64_t T = qkv.size(0);
+    for (const Tensor* w : {&wq, &bq, &wk, &bk})
+        TORCH_CHECK(w->is_contiguous() && w->numel() == hd, what, ": weights and biases must be contiguous [hd]");
+    TORCH_CHECK(mean.is_contiguous() && rstd.is_contiguous() && mean.numel() == T * 2 * H && rstd.numel() == T * 2 * H,
+                what, ": mean / rstd must be contiguous [T * 2 * H]");
+}
 void qk_norm_fwd(Tensor qkv, Tensor wq, Tensor bq, Tensor wk, Tensor bk, Tensor out, Tensor mean, Tensor rstd,
                  int64_t H, int64_t hd, double eps) {
     c10::cuda::CUDAGuard guard(qkv.device());
-    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && out.dim() == 2 && out.stride(1) == 1 &&
-                    out.size(0) == qkv.size(0), "qk_norm_fwd: qkv and out must be row-major [T, 3D] matrices");
-    const int64_t T = qkv.size(0);
-    for (const Tensor* w : {&wq, &bq, &wk, &bk})
-        TORCH_CHECK(w->is_contiguous() && w->numel() == hd, "qk_norm_fwd: weights and biases must be contiguous [hd]");
-    TORCH_CHECK(mean.is_contiguous() && rstd.is_contiguous() && mean.numel() == T * 2 * H && rstd.numel() == T * 2 * H,
-                "qk_norm_fwd: mean / rstd must be contiguous [T * 2 * H]");
+    check_qk_norm_fwd("qk_norm_fwd", qkv, wq, bq, wk, bk, out, mean, rstd, H, hd);
     b200::qk_norm_fwd(bf16_ptr(qkv), qkv.stride(0), bf16_ptr(wq), bf16_ptr(bq), bf16_ptr(wk), bf16_ptr(bk),
-                      bf16_mut(out), out.stride(0), f32_ptr(mean), f32_ptr(rstd), (int)T, (int)H, (int)hd, (float)eps,
-                      cur_stream());
+                      bf16_mut(out), out.stride(0), f32_ptr(mean), f32_ptr(rstd), (int)qkv.size(0), (int)H, (int)hd,
+                      (float)eps, cur_stream());
+}
+void check_qk_norm_bwd(const char* what, const Tensor& dqkv, const Tensor& qkv, const Tensor& wq, const Tensor& wk,
+                       const Tensor& mean, const Tensor& rstd, const Tensor& dwq, const Tensor& dbq, const Tensor& dwk,
+                       const Tensor& dbk, const Tensor& colsum, int64_t H, int64_t hd) {
+    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && dqkv.dim() == 2 && dqkv.stride(1) == 1 &&
+                    dqkv.size(0) == qkv.size(0), what, ": qkv and dqkv must be row-major [T, 3D] matrices");
+    const int64_t T = qkv.size(0);
+    TORCH_CHECK(wq.is_contiguous() && wk.is_contiguous() && wq.numel() == hd && wk.numel() == hd,
+                what, ": weights must be contiguous [hd]");
+    TORCH_CHECK(mean.is_contiguous() && rstd.is_contiguous() && mean.numel() == T * 2 * H && rstd.numel() == T * 2 * H,
+                what, ": mean / rstd must be contiguous [T * 2 * H]");
+    for (const Tensor* a : {&dwq, &dbq, &dwk, &dbk})
+        TORCH_CHECK(a->is_contiguous() && a->numel() == hd, what, ": dw / db must be contiguous fp32 [hd]");
+    TORCH_CHECK(colsum.is_contiguous() && colsum.numel() >= 2 * H * hd, what, ": colsum must be fp32 [>= 2 H hd]");
 }
 void qk_norm_bwd(Tensor dqkv, Tensor qkv, Tensor wq, Tensor wk, Tensor mean, Tensor rstd, Tensor dwq, Tensor dbq,
                  Tensor dwk, Tensor dbk, Tensor colsum, int64_t H, int64_t hd) {
     c10::cuda::CUDAGuard guard(qkv.device());
-    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && dqkv.dim() == 2 && dqkv.stride(1) == 1 &&
-                    dqkv.size(0) == qkv.size(0), "qk_norm_bwd: qkv and dqkv must be row-major [T, 3D] matrices");
-    const int64_t T = qkv.size(0);
-    TORCH_CHECK(wq.is_contiguous() && wk.is_contiguous() && wq.numel() == hd && wk.numel() == hd,
-                "qk_norm_bwd: weights must be contiguous [hd]");
-    TORCH_CHECK(mean.is_contiguous() && rstd.is_contiguous() && mean.numel() == T * 2 * H && rstd.numel() == T * 2 * H,
-                "qk_norm_bwd: mean / rstd must be contiguous [T * 2 * H]");
-    for (const Tensor* a : {&dwq, &dbq, &dwk, &dbk})
-        TORCH_CHECK(a->is_contiguous() && a->numel() == hd, "qk_norm_bwd: dw / db must be contiguous fp32 [hd]");
-    TORCH_CHECK(colsum.is_contiguous() && colsum.numel() >= 2 * H * hd, "qk_norm_bwd: colsum must be fp32 [>= 2 H hd]");
+    check_qk_norm_bwd("qk_norm_bwd", dqkv, qkv, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, colsum, H, hd);
     b200::qk_norm_bwd(bf16_mut(dqkv), dqkv.stride(0), bf16_ptr(qkv), qkv.stride(0), bf16_ptr(wq), bf16_ptr(wk),
                       f32_ptr(mean), f32_ptr(rstd), f32_ptr(dwq), f32_ptr(dbq), f32_ptr(dwk), f32_ptr(dbk),
-                      f32_ptr(colsum), (int)T, (int)H, (int)hd, cur_stream());
+                      f32_ptr(colsum), (int)qkv.size(0), (int)H, (int)hd, cur_stream());
+}
+
+// Rotary position embedding on the [rows, >= 3 H hd] qkv buffer of B images: cos / sin contiguous fp32 [N, hd / 2] CUDA
+// tables, keep (optional) contiguous int32 [B, rows / B - P] table rows of the patch tokens.
+b200::RopeArgs make_rope(const char* what, int64_t rows, const Tensor& cos, const Tensor& sin, const OptT& keep,
+                         int64_t B, int64_t P, int64_t hd) {
+    TORCH_CHECK(B >= 1 && rows % B == 0, what, ": the ", rows, " rows are not B = ", B, " images of equal length");
+    const int64_t T = rows / B;
+    TORCH_CHECK(P >= 0 && P <= T, what, ": need 0 <= P <= T, got P ", P, ", T ", T);
+    TORCH_CHECK(T <= INT_MAX && rows <= INT_MAX, what, ": rows B * T = ", rows, " overflow 32 bits");
+    for (const Tensor* t : {&cos, &sin})
+        TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kFloat && t->dim() == 2 && t->is_contiguous() &&
+                        t->size(1) * 2 == hd && t->sizes() == cos.sizes(),
+                    what, ": cos / sin tables must be contiguous fp32 CUDA [N, hd / 2] of one shape, got ",
+                    t->sizes(), " for hd ", hd);
+    b200::RopeArgs r;
+    r.cos = cos.data_ptr<float>(), r.sin = sin.data_ptr<float>();
+    r.tokens = (int)T, r.prefix = (int)P;
+    TORCH_CHECK(cos.size(0) <= INT_MAX, what, ": table rows overflow 32 bits");
+    r.n_tab = (int)cos.size(0);
+    if (keep.has_value()) {
+        TORCH_CHECK(keep->is_cuda() && keep->scalar_type() == at::kInt && keep->is_contiguous(), what,
+                    ": keep must be a contiguous int32 CUDA tensor");
+        TORCH_CHECK(keep->dim() == 2 && keep->size(0) == B && keep->size(1) == T - P, what, ": keep must be [B, T - P] = [",
+                    B, ", ", T - P, "], got ", keep->sizes());
+        r.keep = keep->data_ptr<int>();
+    }
+    return r;
+}
+void rope_fwd(Tensor qkv, Tensor out, Tensor cos, Tensor sin, OptT keep, int64_t B, int64_t P, int64_t H, int64_t hd) {
+    c10::cuda::CUDAGuard guard(qkv.device());
+    TORCH_CHECK(qkv.dim() == 2 && qkv.stride(1) == 1 && out.dim() == 2 && out.stride(1) == 1 &&
+                    out.size(0) == qkv.size(0), "rope_fwd: qkv and out must be row-major [T, 3D] matrices");
+    const b200::RopeArgs r = make_rope("rope_fwd", qkv.size(0), cos, sin, keep, B, P, hd);
+    b200::rope_fwd(bf16_ptr(qkv), qkv.stride(0), bf16_mut(out), out.stride(0), r, (int)B, (int)H, (int)hd,
+                   cur_stream());
+}
+void rope_bwd(Tensor dqkv, Tensor cos, Tensor sin, OptT keep, Tensor colsum, int64_t B, int64_t P, int64_t H,
+              int64_t hd) {
+    c10::cuda::CUDAGuard guard(dqkv.device());
+    TORCH_CHECK(dqkv.dim() == 2 && dqkv.stride(1) == 1, "rope_bwd: dqkv must be a row-major [T, 3D] matrix");
+    TORCH_CHECK(colsum.is_contiguous() && colsum.numel() == 2 * H * hd, "rope_bwd: colsum must be contiguous fp32 [2D]");
+    const b200::RopeArgs r = make_rope("rope_bwd", dqkv.size(0), cos, sin, keep, B, P, hd);
+    b200::rope_bwd(bf16_mut(dqkv), dqkv.stride(0), r, (int)B, (int)H, (int)hd, f32_ptr(colsum), cur_stream());
+}
+void qk_norm_rope_fwd(Tensor qkv, Tensor wq, Tensor bq, Tensor wk, Tensor bk, Tensor out, Tensor mean, Tensor rstd,
+                      Tensor cos, Tensor sin, OptT keep, int64_t B, int64_t P, int64_t H, int64_t hd, double eps) {
+    c10::cuda::CUDAGuard guard(qkv.device());
+    check_qk_norm_fwd("qk_norm_rope_fwd", qkv, wq, bq, wk, bk, out, mean, rstd, H, hd);
+    const b200::RopeArgs r = make_rope("qk_norm_rope_fwd", qkv.size(0), cos, sin, keep, B, P, hd);
+    b200::qk_norm_rope_fwd(bf16_ptr(qkv), qkv.stride(0), bf16_ptr(wq), bf16_ptr(bq), bf16_ptr(wk), bf16_ptr(bk),
+                           bf16_mut(out), out.stride(0), f32_ptr(mean), f32_ptr(rstd), r, (int)B, (int)H, (int)hd,
+                           (float)eps, cur_stream());
+}
+void qk_norm_rope_bwd(Tensor dqkv, Tensor qkv, Tensor wq, Tensor wk, Tensor mean, Tensor rstd, Tensor dwq, Tensor dbq,
+                      Tensor dwk, Tensor dbk, Tensor colsum, Tensor cos, Tensor sin, OptT keep, int64_t B, int64_t P,
+                      int64_t H, int64_t hd) {
+    c10::cuda::CUDAGuard guard(qkv.device());
+    check_qk_norm_bwd("qk_norm_rope_bwd", dqkv, qkv, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, colsum, H, hd);
+    const b200::RopeArgs r = make_rope("qk_norm_rope_bwd", qkv.size(0), cos, sin, keep, B, P, hd);
+    b200::qk_norm_rope_bwd(bf16_mut(dqkv), dqkv.stride(0), bf16_ptr(qkv), qkv.stride(0), bf16_ptr(wq), bf16_ptr(wk),
+                           f32_ptr(mean), f32_ptr(rstd), f32_ptr(dwq), f32_ptr(dbq), f32_ptr(dwk), f32_ptr(dbk),
+                           f32_ptr(colsum), r, (int)B, (int)H, (int)hd, cur_stream());
 }
 
 // LayerScale folded into a linear layer.  W / dW / Wg: contiguous bf16 [D, K]; b / gamma / bg: contiguous bf16 [D];
@@ -671,6 +746,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     m.def("meanpool_bwd", &meanpool_bwd);
     m.def("qk_norm_fwd", &qk_norm_fwd);
     m.def("qk_norm_bwd", &qk_norm_bwd);
+    m.def("qk_norm_rope_fwd", &qk_norm_rope_fwd);
+    m.def("qk_norm_rope_bwd", &qk_norm_rope_bwd);
+    m.def("rope_fwd", &rope_fwd);
+    m.def("rope_bwd", &rope_bwd);
     m.def("layer_scale_fold", &layer_scale_fold);
     m.def("layer_scale_bwd", &layer_scale_bwd);
     m.def("tokens_fwd", &tokens_fwd);

@@ -17,6 +17,7 @@
 
 #include "elementwise.h"
 #include "ptx.cuh"
+#include "rope.cuh"
 
 namespace b200 {
 
@@ -53,12 +54,13 @@ __device__ __forceinline__ unsigned group_mask() {
 // out[:, 0:2D) = LayerNorm_hd of every q / k head; mean / rstd [T, 2, H].  Out of place (slots == 3H) the v heads are
 // copied to out as they are; in place (out == qkv, slots == 2H) they are not touched.  qkv / out are not __restrict__:
 // in place, every element is read by the lane that later overwrites it, and by no other.
-template <int kVpl>
-__global__ void __launch_bounds__(kQkThreads) qk_norm_fwd_kernel(
+// With kRope the normalised, affine-transformed q / k of a patch row are rotated (rope.cuh) before the one rounding.
+template <int kVpl, bool kRope>
+__device__ __forceinline__ void qk_norm_fwd_body(
     const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* __restrict__ wq, const __nv_bfloat16* __restrict__ bq,
     const __nv_bfloat16* __restrict__ wk, const __nv_bfloat16* __restrict__ bk, __nv_bfloat16* out, int64_t ld_out,
     float* __restrict__ mean_out, float* __restrict__ rstd_out, int T, int H, int hd, int slots, int tokens_per_cta,
-    float eps) {
+    float eps, const RopeArgs& rope) {
     constexpr int kTok = kVpl <= 2 ? 2 : 1;  // tokens whose loads are in flight together
     const int g = threadIdx.x / kQkLanes, lane = threadIdx.x % kQkLanes;
     const int j = blockIdx.x * kQkGroups + g;
@@ -109,6 +111,7 @@ __global__ void __launch_bounds__(kQkThreads) qk_norm_fwd_kernel(
             }
         }
         const float rstd = rsqrtf(group_sum<kQkLanes>(ss, mask) * inv_hd + eps);
+        const int n = kRope ? rope_row(rope, static_cast<int>(t)) : -1;
 #pragma unroll
         for (int i = 0; i < kVpl; ++i) {
             const int idx = lane + i * kQkLanes;
@@ -119,6 +122,7 @@ __global__ void __launch_bounds__(kQkThreads) qk_norm_fwd_kernel(
                 qk_unpack8(bt[i], b);
 #pragma unroll
                 for (int q = 0; q < 8; ++q) f[q] = (f[q] - mean) * rstd * w[q] + b[q];
+                if (kRope && n >= 0) rope_rotate<false>(f, rope, n, hd / 2, idx * 4);
                 reinterpret_cast<uint4*>(dst)[idx] = qk_pack8(f);
             }
         }
@@ -146,17 +150,39 @@ __global__ void __launch_bounds__(kQkThreads) qk_norm_fwd_kernel(
     }
 }
 
+template <int kVpl>
+__global__ void __launch_bounds__(kQkThreads) qk_norm_fwd_kernel(
+    const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* __restrict__ wq, const __nv_bfloat16* __restrict__ bq,
+    const __nv_bfloat16* __restrict__ wk, const __nv_bfloat16* __restrict__ bk, __nv_bfloat16* out, int64_t ld_out,
+    float* __restrict__ mean_out, float* __restrict__ rstd_out, int T, int H, int hd, int slots, int tokens_per_cta,
+    float eps) {
+    qk_norm_fwd_body<kVpl, false>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean_out, rstd_out, T, H, hd, slots,
+                                  tokens_per_cta, eps, RopeArgs());
+}
+template <int kVpl>
+__global__ void __launch_bounds__(kQkThreads) qk_norm_rope_fwd_kernel(
+    const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* __restrict__ wq, const __nv_bfloat16* __restrict__ bq,
+    const __nv_bfloat16* __restrict__ wk, const __nv_bfloat16* __restrict__ bk, __nv_bfloat16* out, int64_t ld_out,
+    float* __restrict__ mean_out, float* __restrict__ rstd_out, int T, int H, int hd, int slots, int tokens_per_cta,
+    float eps, RopeArgs rope) {
+    qk_norm_fwd_body<kVpl, true>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean_out, rstd_out, T, H, hd, slots,
+                                 tokens_per_cta, eps, rope);
+}
+
 // In place on dqkv[:, 0:2D): the gradient of the normalised q / k becomes that of the un-normalised q / k (the standard
 // LayerNorm backward on xhat = (x - mean) * rstd, x read from qkv).  dw / db: fp32 [hd] sums over all T * H rows of the
 // side, reduced per CTA in shared memory and added with one atomic per column per CTA.  colsum[0, 2D): fp32 column sums
 // of the stored bf16 dq / dk (the q / k part of the qkv bias gradient); every group of a CTA owns its own head slot, so
 // each column gets one atomic per CTA.  All accumulators are added to: zero them first.
-template <int kLanes, int kVpl>
-__global__ void __launch_bounds__(kQkThreads) qk_norm_bwd_kernel(
+// With kRope the incoming dq / dk of a patch row are the gradients of the rotated values: R^T turns them, in fp32
+// registers, into the gradients of the normalised ones before anything else reads them.
+template <int kLanes, int kVpl, bool kRope>
+__device__ __forceinline__ void qk_norm_bwd_body(
     __nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* __restrict__ qkv, int64_t ld,
     const __nv_bfloat16* __restrict__ wq, const __nv_bfloat16* __restrict__ wk, const float* __restrict__ mean,
     const float* __restrict__ rstd, float* __restrict__ dwq, float* __restrict__ dbq, float* __restrict__ dwk,
-    float* __restrict__ dbk, float* __restrict__ colsum, int T, int H, int hd, int tokens_per_cta) {
+    float* __restrict__ dbk, float* __restrict__ colsum, int T, int H, int hd, int tokens_per_cta,
+    const RopeArgs& rope) {
     constexpr int kGroups = kQkThreads / kLanes;
     __shared__ float red[4][kQkMaxHd];  // dw_q, db_q, dw_k, db_k of this CTA
     for (int i = threadIdx.x; i < 4 * kQkMaxHd; i += kQkThreads) (&red[0][0])[i] = 0.f;
@@ -184,12 +210,14 @@ __global__ void __launch_bounds__(kQkThreads) qk_norm_bwd_kernel(
 
         auto row = [&](const uint4 (&xv)[kVpl], const uint4 (&dv)[kVpl], int64_t t) {
             const float m = __ldg(mean + t * 2 * H + j), r = __ldg(rstd + t * 2 * H + j);
+            const int n = kRope ? rope_row(rope, static_cast<int>(t)) : -1;
             float s1 = 0.f, s2 = 0.f;
 #pragma unroll
             for (int i = 0; i < kVpl; ++i) {
                 float x[8], dy[8], w[8];
                 qk_unpack8(xv[i], x);
                 qk_unpack8(dv[i], dy);  // zero past the head: those columns add nothing
+                if (kRope && n >= 0 && lane + i * kLanes < nvec) rope_rotate<true>(dy, rope, n, hd / 2, (lane + i * kLanes) * 4);
                 qk_unpack8(gm[i], w);
 #pragma unroll
                 for (int q = 0; q < 8; ++q) {
@@ -210,6 +238,7 @@ __global__ void __launch_bounds__(kQkThreads) qk_norm_bwd_kernel(
                     float x[8], dy[8], w[8];
                     qk_unpack8(xv[i], x);
                     qk_unpack8(dv[i], dy);
+                    if (kRope && n >= 0) rope_rotate<true>(dy, rope, n, hd / 2, idx * 4);
                     qk_unpack8(gm[i], w);
 #pragma unroll
                     for (int q = 0; q < 8; ++q) dy[q] = r * (dy[q] * w[q] - s1 - (x[q] - m) * r * s2);
@@ -260,6 +289,25 @@ __global__ void __launch_bounds__(kQkThreads) qk_norm_bwd_kernel(
     }
 }
 
+template <int kLanes, int kVpl>
+__global__ void __launch_bounds__(kQkThreads) qk_norm_bwd_kernel(
+    __nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* __restrict__ qkv, int64_t ld,
+    const __nv_bfloat16* __restrict__ wq, const __nv_bfloat16* __restrict__ wk, const float* __restrict__ mean,
+    const float* __restrict__ rstd, float* __restrict__ dwq, float* __restrict__ dbq, float* __restrict__ dwk,
+    float* __restrict__ dbk, float* __restrict__ colsum, int T, int H, int hd, int tokens_per_cta) {
+    qk_norm_bwd_body<kLanes, kVpl, false>(dqkv, ld_d, qkv, ld, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, colsum, T, H, hd,
+                                          tokens_per_cta, RopeArgs());
+}
+template <int kLanes, int kVpl>
+__global__ void __launch_bounds__(kQkThreads, 2) qk_norm_rope_bwd_kernel(  // two CTAs per SM, as the plain kernel
+    __nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* __restrict__ qkv, int64_t ld,
+    const __nv_bfloat16* __restrict__ wq, const __nv_bfloat16* __restrict__ wk, const float* __restrict__ mean,
+    const float* __restrict__ rstd, float* __restrict__ dwq, float* __restrict__ dbq, float* __restrict__ dwk,
+    float* __restrict__ dbk, float* __restrict__ colsum, int T, int H, int hd, int tokens_per_cta, RopeArgs rope) {
+    qk_norm_bwd_body<kLanes, kVpl, true>(dqkv, ld_d, qkv, ld, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, colsum, T, H, hd,
+                                         tokens_per_cta, rope);
+}
+
 inline void check_launch_qk(const char* what) {
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(err));
@@ -300,42 +348,56 @@ void qk_grid(int T, int gx, int ctas, int& slabs, int& tokens_per) {
 
 }  // namespace
 
-void qk_norm_fwd(const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* wq, const __nv_bfloat16* bq,
-                 const __nv_bfloat16* wk, const __nv_bfloat16* bk, __nv_bfloat16* out, int64_t ld_out, float* mean,
-                 float* rstd, int T, int H, int hd, float eps, cudaStream_t stream) {
-    check_qk_shapes("qk_norm_fwd", T, H, hd);
+namespace {
+
+// rope == nullptr: the plain kernels; otherwise the RoPE-fused instances, with B images of rope->tokens rows.
+void qk_norm_fwd_launch(const char* what, const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* wq,
+                        const __nv_bfloat16* bq, const __nv_bfloat16* wk, const __nv_bfloat16* bk, __nv_bfloat16* out,
+                        int64_t ld_out, float* mean, float* rstd, int T, int H, int hd, float eps,
+                        const RopeArgs* rope, cudaStream_t stream) {
+    check_qk_shapes(what, T, H, hd);
     const int64_t width = 3 * static_cast<int64_t>(H) * hd;
-    check_qk_matrix("qk_norm_fwd", "qkv", qkv, ld, width);
-    check_qk_matrix("qk_norm_fwd", "out", out, ld_out, width);
+    check_qk_matrix(what, "qkv", qkv, ld, width);
+    check_qk_matrix(what, "out", out, ld_out, width);
     for (const void* p : {static_cast<const void*>(wq), static_cast<const void*>(bq), static_cast<const void*>(wk),
                           static_cast<const void*>(bk)})
-        if (reinterpret_cast<uintptr_t>(p) & 15) throw std::runtime_error("qk_norm_fwd: weights must be 16-byte aligned");
+        if (reinterpret_cast<uintptr_t>(p) & 15) throw std::runtime_error(std::string(what) + ": weights must be 16-byte aligned");
     const bool in_place = out == qkv;
-    if (in_place && ld_out != ld) throw std::runtime_error("qk_norm_fwd: in place needs ld_out == ld");
+    if (in_place && ld_out != ld) throw std::runtime_error(std::string(what) + ": in place needs ld_out == ld");
     if (T == 0) return;
     const int slots = (in_place ? 2 : 3) * H;
     const int gx = (slots + kQkGroups - 1) / kQkGroups;
     int slabs, tokens_per;
     qk_grid(T, gx, sm_count_qk() * 32, slabs, tokens_per);
     const dim3 grid(gx, slabs);
-    switch ((hd / 8 + kQkLanes - 1) / kQkLanes) {
-        case 1: qk_norm_fwd_kernel<1><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps); break;
-        case 2: qk_norm_fwd_kernel<2><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps); break;
-        case 3: qk_norm_fwd_kernel<3><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps); break;
-        default: qk_norm_fwd_kernel<4><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps); break;
+    if (rope) {
+        switch ((hd / 8 + kQkLanes - 1) / kQkLanes) {
+            case 1: qk_norm_rope_fwd_kernel<1><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps, *rope); break;
+            case 2: qk_norm_rope_fwd_kernel<2><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps, *rope); break;
+            case 3: qk_norm_rope_fwd_kernel<3><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps, *rope); break;
+            default: qk_norm_rope_fwd_kernel<4><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps, *rope); break;
+        }
+    } else {
+        switch ((hd / 8 + kQkLanes - 1) / kQkLanes) {
+            case 1: qk_norm_fwd_kernel<1><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps); break;
+            case 2: qk_norm_fwd_kernel<2><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps); break;
+            case 3: qk_norm_fwd_kernel<3><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps); break;
+            default: qk_norm_fwd_kernel<4><<<grid, kQkThreads, 0, stream>>>(qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, slots, tokens_per, eps); break;
+        }
     }
-    check_launch_qk("qk_norm_fwd");
+    check_launch_qk(what);
 }
 
-void qk_norm_bwd(__nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* wq,
-                 const __nv_bfloat16* wk, const float* mean, const float* rstd, float* dwq, float* dbq, float* dwk,
-                 float* dbk, float* colsum, int T, int H, int hd, cudaStream_t stream) {
-    check_qk_shapes("qk_norm_bwd", T, H, hd);
+void qk_norm_bwd_launch(const char* what, __nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* qkv, int64_t ld,
+                        const __nv_bfloat16* wq, const __nv_bfloat16* wk, const float* mean, const float* rstd,
+                        float* dwq, float* dbq, float* dwk, float* dbk, float* colsum, int T, int H, int hd,
+                        const RopeArgs* rope, cudaStream_t stream) {
+    check_qk_shapes(what, T, H, hd);
     const int64_t width = 3 * static_cast<int64_t>(H) * hd;
-    check_qk_matrix("qk_norm_bwd", "dqkv", dqkv, ld_d, width);
-    check_qk_matrix("qk_norm_bwd", "qkv", qkv, ld, width);
+    check_qk_matrix(what, "dqkv", dqkv, ld_d, width);
+    check_qk_matrix(what, "qkv", qkv, ld, width);
     if ((reinterpret_cast<uintptr_t>(wq) | reinterpret_cast<uintptr_t>(wk)) & 15)
-        throw std::runtime_error("qk_norm_bwd: weights must be 16-byte aligned");
+        throw std::runtime_error(std::string(what) + ": weights must be 16-byte aligned");
     if (T == 0) return;
     // Three builds keep the three fp32 accumulators of each lane (dw, db, colsum) in at most 2 x 8 columns, so that two
     // CTAs fit an SM without spills: 8 lanes x 1 vector (hd <= 64), 8 x 2 (hd <= 128), 16 x 2 (hd <= 256).
@@ -346,11 +408,54 @@ void qk_norm_bwd(__nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* qkv, in
     qk_grid(T, gx, sm_count_qk() * 2, slabs, tokens_per);  // one resident wave: few dw / db atomics
     const dim3 grid(gx, slabs);
 #define QK_BWD(L, V) qk_norm_bwd_kernel<L, V><<<grid, kQkThreads, 0, stream>>>(dqkv, ld_d, qkv, ld, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, colsum, T, H, hd, tokens_per)
-    if (nvec <= 8) QK_BWD(8, 1);
-    else if (nvec <= 16) QK_BWD(8, 2);
-    else QK_BWD(16, 2);
+#define QK_ROPE_BWD(L, V) qk_norm_rope_bwd_kernel<L, V><<<grid, kQkThreads, 0, stream>>>(dqkv, ld_d, qkv, ld, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, colsum, T, H, hd, tokens_per, *rope)
+    if (rope) {
+        if (nvec <= 8) QK_ROPE_BWD(8, 1);
+        else if (nvec <= 16) QK_ROPE_BWD(8, 2);
+        else QK_ROPE_BWD(16, 2);
+    } else {
+        if (nvec <= 8) QK_BWD(8, 1);
+        else if (nvec <= 16) QK_BWD(8, 2);
+        else QK_BWD(16, 2);
+    }
+#undef QK_ROPE_BWD
 #undef QK_BWD
-    check_launch_qk("qk_norm_bwd");
+    check_launch_qk(what);
+}
+
+}  // namespace
+
+void qk_norm_fwd(const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* wq, const __nv_bfloat16* bq,
+                 const __nv_bfloat16* wk, const __nv_bfloat16* bk, __nv_bfloat16* out, int64_t ld_out, float* mean,
+                 float* rstd, int T, int H, int hd, float eps, cudaStream_t stream) {
+    qk_norm_fwd_launch("qk_norm_fwd", qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, eps, nullptr, stream);
+}
+
+void qk_norm_bwd(__nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* wq,
+                 const __nv_bfloat16* wk, const float* mean, const float* rstd, float* dwq, float* dbq, float* dwk,
+                 float* dbk, float* colsum, int T, int H, int hd, cudaStream_t stream) {
+    qk_norm_bwd_launch("qk_norm_bwd", dqkv, ld_d, qkv, ld, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, colsum, T, H, hd,
+                       nullptr, stream);
+}
+
+void qk_norm_rope_fwd(const __nv_bfloat16* qkv, int64_t ld, const __nv_bfloat16* wq, const __nv_bfloat16* bq,
+                      const __nv_bfloat16* wk, const __nv_bfloat16* bk, __nv_bfloat16* out, int64_t ld_out,
+                      float* mean, float* rstd, const RopeArgs& rope, int B, int H, int hd, float eps,
+                      cudaStream_t stream) {
+    check_rope_args("qk_norm_rope_fwd", rope, B, H, hd);  // also: B * tokens fits 32 bits
+    const int T = B * rope.tokens;
+    qk_norm_fwd_launch("qk_norm_rope_fwd", qkv, ld, wq, bq, wk, bk, out, ld_out, mean, rstd, T, H, hd, eps, &rope,
+                       stream);
+}
+
+void qk_norm_rope_bwd(__nv_bfloat16* dqkv, int64_t ld_d, const __nv_bfloat16* qkv, int64_t ld,
+                      const __nv_bfloat16* wq, const __nv_bfloat16* wk, const float* mean, const float* rstd,
+                      float* dwq, float* dbq, float* dwk, float* dbk, float* colsum, const RopeArgs& rope, int B,
+                      int H, int hd, cudaStream_t stream) {
+    check_rope_args("qk_norm_rope_bwd", rope, B, H, hd);  // also: B * tokens fits 32 bits
+    const int T = B * rope.tokens;
+    qk_norm_bwd_launch("qk_norm_rope_bwd", dqkv, ld_d, qkv, ld, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, colsum, T, H,
+                       hd, &rope, stream);
 }
 
 }  // namespace b200

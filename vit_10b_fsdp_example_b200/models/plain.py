@@ -10,6 +10,8 @@ LayerNorm (eps 1e-6), mean pool, linear head.
 With ``cfg.class_token`` it is timm's token layout instead: ``cls_token`` and ``reg_token`` in front of the patches,
 ``pos_embed`` over all tokens (or the patches only, ``cfg.no_embed_class``), and the head on token 0.
 With ``cfg.patch_drop_rate`` it applies timm's ``PatchDropout(ordered=True)`` after ``pos_drop`` in training.
+With ``cfg.rope`` the attention rotates q and k of the patch tokens after ``q_norm`` / ``k_norm`` (EVA-02's 2-D axial
+RoPE, ``vit.rope_tables``), each kept patch at its original position.
 It runs on stock PyTorch ops (any device) and is meant for evaluation / export / fine-tuning outside the engine.
 """
 from __future__ import annotations
@@ -35,13 +37,25 @@ class _Attention(nn.Module):
         self.proj = nn.Linear(dim, dim)
         self.proj_drop = nn.Dropout(proj_drop)
 
-    def forward(self, x):
+    def forward(self, x, rope=None):
+        """rope: (cos, sin, P) with cos / sin [B or 1, N - P, hd / 2], the angles of the patch tokens."""
         B, N, C = x.shape
         q, k, v = self.qkv(x).reshape(B, N, 3, self.num_heads, C // self.num_heads).permute(2, 0, 3, 1, 4)
         if self.q_norm is not None:
             q, k = self.q_norm(q), self.k_norm(k)
+        if rope is not None:
+            q, k = _rotate(q, *rope), _rotate(k, *rope)
         o = F.scaled_dot_product_attention(q, k, v, dropout_p=self.attn_drop if self.training else 0.0)
         return self.proj_drop(self.proj(o.transpose(1, 2).reshape(B, N, C)))
+
+
+def _rotate(x, cos, sin, P: int):
+    """x [B, H, N, hd]: the interleaved pairs (2i, 2i + 1) of tokens P.. turn by the angles of cos / sin."""
+    c, s = cos.unsqueeze(1).to(x.dtype), sin.unsqueeze(1).to(x.dtype)  # [B or 1, 1, N - P, hd / 2]
+    xp = x[:, :, P:].unflatten(-1, (-1, 2))
+    x0, x1 = xp[..., 0], xp[..., 1]
+    y = torch.stack((x0 * c - x1 * s, x1 * c + x0 * s), dim=-1).flatten(-2)
+    return torch.cat((x[:, :, :P], y), dim=2)
 
 
 class _Mlp(nn.Module):
@@ -95,8 +109,8 @@ class _Block(nn.Module):
         self.mlp = (_GluMlp if cfg.swiglu else _Mlp)(cfg.embed_dim, cfg.hidden_dim, cfg.mlp_dropout)
         self.ls2 = _LayerScale(cfg.embed_dim, cfg.init_values) if cfg.init_values else nn.Identity()
 
-    def forward(self, x):
-        x = x + self.ls1(self.attn(self.norm1(x)))
+    def forward(self, x, rope=None):
+        x = x + self.ls1(self.attn(self.norm1(x), rope))
         return x + self.ls2(self.mlp(self.norm2(x)))
 
 
@@ -118,6 +132,11 @@ class _PatchDropout(nn.Module):
         super().__init__()
         self.prob, self.num_prefix_tokens = prob, num_prefix_tokens
 
+    def draw(self, B: int, L: int, device):
+        """timm's random subset: [B, K] kept patches, ascending."""
+        num_keep = max(1, int(L * (1.0 - self.prob)))
+        return torch.argsort(torch.randn(B, L, device=device), dim=-1)[:, :num_keep].sort(dim=-1)[0]
+
     def forward(self, x, keep=None):
         if not self.training or self.prob == 0.0:
             return x
@@ -125,8 +144,7 @@ class _PatchDropout(nn.Module):
         prefix, x = x[:, :P], x[:, P:]
         B, L = x.shape[:2]
         if keep is None:
-            num_keep = max(1, int(L * (1.0 - self.prob)))
-            keep = torch.argsort(torch.randn(B, L, device=x.device), dim=-1)[:, :num_keep].sort(dim=-1)[0]
+            keep = self.draw(B, L, x.device)
         x = x.gather(1, keep.long().unsqueeze(-1).expand(-1, -1, x.shape[-1]))
         return torch.cat((prefix, x), dim=1) if P else x
 
@@ -145,12 +163,37 @@ class PlainViT(nn.Module):
         self.blocks = nn.Sequential(*[_Block(cfg) for _ in range(cfg.num_blocks)])
         self.norm = nn.LayerNorm(cfg.embed_dim, eps=1e-6)
         self.head = nn.Linear(cfg.embed_dim, cfg.num_classes)
+        if cfg.rope:  # no parameters: buffers kept out of the state_dict
+            from .vit import rope_tables
+            cos, sin = rope_tables(cfg.grid, cfg.head_dim, cfg.rope_theta, cfg.rope_ref_grid)
+            self.register_buffer("rope_cos", cos, persistent=False)
+            self.register_buffer("rope_sin", sin, persistent=False)
+
+    def _rope(self, patch_keep):
+        """(cos, sin, P) of the patch tokens the blocks see: the full grid, or the kept patches' rows."""
+        if not self.cfg.rope:
+            return None
+        cos, sin = self.rope_cos[None], self.rope_sin[None]
+        if patch_keep is not None and self.training and self.cfg.patch_drop_rate > 0:
+            idx = patch_keep.long()
+            cos, sin = self.rope_cos[idx], self.rope_sin[idx]
+        return cos, sin, self.cfg.num_prefix_tokens
+
+    def _blocks(self, x, patch_keep):
+        rope = self._rope(patch_keep)
+        if rope is None:
+            return self.blocks(x)
+        for blk in self.blocks:
+            x = blk(x, rope)
+        return x
 
     def forward(self, image, patch_keep=None):
         """patch_keep: optional [B, K] kept patches of the patch dropout (training only)."""
+        if self.cfg.rope and patch_keep is None and self.training and self.cfg.patch_drop_rate > 0:
+            patch_keep = self.patch_drop.draw(image.shape[0], self.cfg.num_patches, image.device)  # RoPE needs them
         if self.cls_token is None:
             x = self.patch_drop(self.pos_drop(self.patch_embed(image) + self.pos_embed), patch_keep)
-            x = self.blocks(x)
+            x = self._blocks(x, patch_keep)
             return self.head(self.norm(x).mean(dim=1))
         x = self.patch_embed(image)
         prefix = [self.cls_token.expand(x.shape[0], -1, -1)]
@@ -160,7 +203,7 @@ class PlainViT(nn.Module):
             x = torch.cat(prefix + [x + self.pos_embed], dim=1)
         else:
             x = torch.cat(prefix + [x], dim=1) + self.pos_embed
-        x = self.blocks(self.patch_drop(self.pos_drop(x), patch_keep))
+        x = self._blocks(self.patch_drop(self.pos_drop(x), patch_keep), patch_keep)
         return self.head(self.norm(x)[:, 0])
 
     @classmethod

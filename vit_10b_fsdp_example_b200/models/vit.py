@@ -27,6 +27,10 @@ Architecture parity with the reference model (run_vit_training.py:99-162, timm 0
     training every image keeps K = max(1, int(N * (1 - R))) of its patches, drawn on the GPU (ops.patch_drop_select);
     only they go through the im2col and the patch GEMM, with their own pos_embed rows, and every block runs on
     T' = P + K tokens.  Evaluation keeps all patches
+  * optional rotary position embedding (EVA-02, timm Eva(use_rot_pos_emb=True) with RotaryEmbeddingCat, off in the
+    reference): q and k of every head, after the QK norm, are rotated pair by pair by their patch's position
+    (``rope_tables``); prefix tokens are not rotated, and under patch dropout a kept patch keeps its original position.
+    No parameters: the learned pos_embed stays
   * final LayerNorm(eps=1e-6), mean-pool over tokens (no CLS token), Linear head      (:151-153,159-161);
     with a class token: LayerNorm of the B class rows only (it acts per row) and the head on them
 Parameter names are timm-compatible (``norm1.weight``, ``attn.qkv.weight``, ``mlp.fc1.bias`` ...).
@@ -40,7 +44,7 @@ from __future__ import annotations
 
 import functools
 import math
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -223,10 +227,42 @@ def drop_path_rates(cfg: ViTConfig) -> List[float]:
 
 
 # ------------------------------------------------------------------------------------------------
+# Rotary position embedding (--rope): 2-D axial RoPE, timm RotaryEmbeddingCat as Eva uses it (EVA-02)
+# ------------------------------------------------------------------------------------------------
+def rope_tables(grid: int, hd: int, theta: float, ref_grid: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(cos, sin) fp32 [grid * grid, hd / 2], computed in float64.  Patch n sits at row r = n // grid, column
+    c = n % grid, at positions t_r = r * g_ref / grid and t_c = c * g_ref / grid (g_ref = ref_grid, or grid at 0: timm's
+    ref_feat_shape).  With F = hd / 4 and w_j = theta ** (-j / F), pair i < F turns by t_r * w_i and pair i >= F by
+    t_c * w_(i - F)."""
+    if hd % 4:
+        raise ValueError(f"RoPE needs head_dim % 4 == 0, got {hd}")
+    F = hd // 4
+    g_ref = ref_grid or grid
+    n = np.arange(grid * grid, dtype=np.float64)
+    t_r, t_c = (n // grid) * g_ref / grid, (n % grid) * g_ref / grid
+    w = float(theta) ** (-np.arange(F, dtype=np.float64) / F)
+    ang = np.concatenate([t_r[:, None] * w[None, :], t_c[:, None] * w[None, :]], axis=1)
+    return torch.from_numpy(np.cos(ang).astype(np.float32)), torch.from_numpy(np.sin(ang).astype(np.float32))
+
+
+class Rope(NamedTuple):
+    """What a block's rotation needs: the tables of ``rope_tables`` on the device, the P prefix tokens (not rotated)
+    and, after patch dropout, the kept patches' original indices keep [B, K] (their table rows)."""
+    cos: torch.Tensor
+    sin: torch.Tensor
+    P: int
+    keep: Optional[torch.Tensor] = None
+
+    def args(self, B: int):
+        """(cos, sin, B, P, keep): the trailing arguments of ops.rope_fwd / rope_bwd and the ops' ``rope=``."""
+        return self.cos, self.sin, B, self.P, self.keep
+
+
+# ------------------------------------------------------------------------------------------------
 # Transformer block
 # ------------------------------------------------------------------------------------------------
 def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[DropoutCtx] = None,
-                  block_idx: int = 0):
+                  block_idx: int = 0, rope: Optional[Rope] = None):
     """x: [B*N, D] -> y: [B*N, D].  With save=True also returns the tensors backward needs; save="lean" keeps
     only what a GEMM would have to recompute (x, qkv, attention output, x1, fc1 pre-activation: 10 [T, D] units
     instead of ~17.6) and block_backward re-materialises h1 / P / h2 / gelu(u) with memory-bound kernels.
@@ -237,7 +273,10 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     A forward that saves nothing normalises in place.
     With prefix tokens every image has cfg.num_tokens rows (class and register tokens first); the block is unchanged.
     The tokens per image are x.shape[0] // B: T' = P + K in a training step with patch dropout.
-    With cfg.swiglu, u is the packed [T, Hd] fc1 pre-activation [gate | value] and g = silu(gate) * value [T, Hd / 2]."""
+    With cfg.swiglu, u is the packed [T, Hd] fc1 pre-activation [gate | value] and g = silu(gate) * value [T, Hd / 2].
+    rope (cfg.rope): without QK normalisation qkv is rotated in place right after the qkv GEMM, so the lean set's qkv is
+    the rotated buffer the attention backward reads; with it the fused qk_norm kernels rotate qkn and the lean set is
+    unchanged (un-normalised, un-rotated qkv and the statistics)."""
     do_save = save is not False and save is not None
     if save is True:
         extras = frozenset(("P", "h", "g"))
@@ -262,9 +301,11 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     ag = getattr(p, "ag", None) or {}  # weights whose all-gather is fused into the GEMM that consumes them
     h1, m1, r1 = ops.ln_fwd(x, p["norm1.weight"], p["norm1.bias"], BLOCK_LN_EPS)
     qkv = ops.linear_fwd(h1, p["attn.qkv.weight"], p["attn.qkv.bias"], ag=ag.get("attn.qkv.weight"))
-    qkn = qkv  # what the attention reads: qkv, or with QK normalisation its normalised copy
+    if rope is not None and not cfg.qk_norm:
+        qkv = ops.rope_fwd(qkv, H, hd, *rope.args(B), inplace=True)
+    qkn = qkv  # what the attention reads: qkv, or with QK normalisation its normalised (and rotated) copy
     if cfg.qk_norm:
-        qkn, qk_mean, qk_rstd = _qk_norm(ops, cfg, p, qkv, inplace=not do_save)
+        qkn, qk_mean, qk_rstd = _qk_norm(ops, cfg, p, qkv, inplace=not do_save, rope=rope, B=B)
     masks = {}  # site name -> dropout key (the masks themselves are regenerated, never stored)
     lse = None
     if use_drop and pa > 0:
@@ -326,7 +367,7 @@ def block_forward(ops, cfg: ViTConfig, p, x, B: int, save, drop: Optional[Dropou
     return y, saved
 
 
-def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
+def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int, rope: Optional[Rope] = None):
     """Backward of one block.
 
     p / G: parameter and gradient views of this unit.  dy_colsum = column sums of dy (fp32), which *is*
@@ -335,6 +376,8 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     With LayerScale the proj / fc2 bias gradient is gamma o colsum instead; the wgrad runs first, then
     ``ops.layer_scale_bwd`` rescales its result and yields the bias and gamma gradients, and the dgrad uses the
     folded weight.
+    With rope the attention backward yields the gradient of the rotated q / k; R^T (ops.rope_bwd, or inside the fused
+    qk_norm backward) turns it into that of the qkv GEMM's output, whose column sums are the q / k bias gradient.
     """
     N, H, hd = s["x"].shape[0] // B, cfg.num_heads, cfg.head_dim
     pa, pm = cfg.att_dropout, cfg.mlp_dropout
@@ -401,7 +444,7 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
     if cfg.qk_norm:
         qkn = s.pop("qkn", None)
         if qkn is None:  # not kept: rebuild the normalised copy the attention read
-            qkn = _qk_norm(ops, cfg, p, s["qkv"], inplace=False)[0]
+            qkn = _qk_norm(ops, cfg, p, s["qkv"], inplace=False, rope=rope, B=B)[0]
     if s.get("lse") is not None:  # flash-style: P (and the dropout mask) is rebuilt inside the fused backward kernels
         dqkv, dbqkv = ops.attention_bwd_lse(da, qkn, s["a"], s["lse"], B, N, H, hd, want_colsum=True,
                                             drop=(pa, masks["att"]) if "att" in masks else None)
@@ -414,12 +457,16 @@ def block_backward(ops, cfg: ViTConfig, p, G, s, dy, dy_colsum, B: int):
         else:
             dqkv, dbqkv = ops.attention_bwd(da, qkn, s["P"], B, N, H, hd, want_colsum=True)
     del da, qkn
+    D = cfg.embed_dim
+    if rope is not None and not cfg.qk_norm:  # the rotation differs per token: the sums must be taken after R^T
+        _, cs = ops.rope_bwd(dqkv, H, hd, *rope.args(B))
+        dbqkv[: 2 * D].copy_(cs)
     if cfg.qk_norm:
         # dq / dk become the gradients of the un-normalised q / k; the bias is added before the norm, so the column
         # sums of the new dq / dk are the q / k part of the qkv bias gradient (dv and its sums are unchanged)
-        D = cfg.embed_dim
+        kw = {} if rope is None else {"rope": rope.args(B)}
         _, dwq, dbq, dwk, dbk, cs = ops.qk_norm_bwd(dqkv, s["qkv"], H, hd, p["attn.q_norm.weight"],
-                                                    p["attn.k_norm.weight"], s["qk_mean"], s["qk_rstd"])
+                                                    p["attn.k_norm.weight"], s["qk_mean"], s["qk_rstd"], **kw)
         dbqkv[: 2 * D].copy_(cs)
         G["attn.q_norm.weight"].copy_(dwq)
         G["attn.q_norm.bias"].copy_(dbq)
@@ -456,9 +503,10 @@ def _layer_scale_bwd(ops, p, G, layer: str, ls: str, colsum):
     return wg
 
 
-def _qk_norm(ops, cfg: ViTConfig, p, qkv, inplace: bool):
+def _qk_norm(ops, cfg: ViTConfig, p, qkv, inplace: bool, rope: Optional[Rope] = None, B: int = 0):
+    kw = {} if rope is None else {"rope": rope.args(B)}
     return ops.qk_norm_fwd(qkv, cfg.num_heads, cfg.head_dim, p["attn.q_norm.weight"], p["attn.q_norm.bias"],
-                           p["attn.k_norm.weight"], p["attn.k_norm.bias"], BLOCK_LN_EPS, inplace=inplace)
+                           p["attn.k_norm.weight"], p["attn.k_norm.bias"], BLOCK_LN_EPS, inplace=inplace, **kw)
 
 
 # ------------------------------------------------------------------------------------------------

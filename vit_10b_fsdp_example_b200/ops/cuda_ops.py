@@ -10,7 +10,9 @@ Every function launches hand-written kernels from ``_C.so``:
     softmax / softmax-backward kernels with materialised P) remains for B200_FUSED_ATTN_BWD=0 and unsupported shapes.
   * LayerNorm fwd/bwd, cross-entropy, im2col, column sums, sum of squares, fused AdamW.
   * QK normalisation: per-head LayerNorm of q and k on the packed qkv buffer and its backward (``qk_norm_fwd`` /
-    ``qk_norm_bwd``, csrc/qk_norm.cu).
+    ``qk_norm_bwd``, csrc/qk_norm.cu), with RoPE-fused instances (``rope=``).
+  * rotary position embedding: 2-D axial RoPE on q and k of the packed qkv buffer and its transpose, which also sums
+    the q / k bias gradient (``rope_fwd`` / ``rope_bwd``, csrc/rope.cu).
   * LayerScale: the per-channel branch scale folded into the proj / fc2 weight and bias, and its backward on the
     weight gradient (``layer_scale_fold`` / ``layer_scale_bwd``, csrc/layer_scale.cu).
   * prefix tokens: the class / register tokens put in front of every image's patch rows, and the backward that splits
@@ -168,25 +170,52 @@ def ln_bwd(dy, x, w, mean, rstd, dres=None, want_dxsum: bool = False):
 # ------------------------------------------------------------------------------------------------
 # QK normalisation (csrc/qk_norm.cu): per-head LayerNorm of q and k on the packed qkv buffer
 # ------------------------------------------------------------------------------------------------
-def qk_norm_fwd(qkv, H: int, hd: int, wq, bq, wk, bk, eps: float, inplace: bool = False):
+def qk_norm_fwd(qkv, H: int, hd: int, wq, bq, wk, bk, eps: float, inplace: bool = False, rope=None):
     """Returns (out, mean, rstd): out = qkv with every q head normalised over hd (weight wq, bias bq) and every k head
     (wk, bk), v unchanged; mean / rstd fp32 [T * 2 * H].  inplace=True writes into qkv itself (the v columns are not
-    touched) and returns it; otherwise out is a new [T, 3D] buffer that also receives a copy of v."""
+    touched) and returns it; otherwise out is a new [T, 3D] buffer that also receives a copy of v.
+    rope = (cos, sin, B, P, keep): the RoPE-fused kernel also rotates the normalised q / k before its one rounding."""
     T = qkv.shape[0]
     out = qkv if inplace else torch.empty(T, 3 * H * hd, dtype=qkv.dtype, device=qkv.device)
     mean = torch.empty(T * 2 * H, dtype=torch.float32, device=qkv.device)
     rstd = torch.empty(T * 2 * H, dtype=torch.float32, device=qkv.device)
-    _C.qk_norm_fwd(qkv, wq, bq, wk, bk, out, mean, rstd, H, hd, float(eps))
+    if rope is None:
+        _C.qk_norm_fwd(qkv, wq, bq, wk, bk, out, mean, rstd, H, hd, float(eps))
+    else:
+        cos, sin, B, P, keep = rope
+        _C.qk_norm_rope_fwd(qkv, wq, bq, wk, bk, out, mean, rstd, cos, sin, keep, int(B), int(P), H, hd, float(eps))
     return out, mean, rstd
 
 
-def qk_norm_bwd(dqkv, qkv, H: int, hd: int, wq, wk, mean, rstd):
+def qk_norm_bwd(dqkv, qkv, H: int, hd: int, wq, wk, mean, rstd, rope=None):
     """In place on dqkv[:, 0:2D); returns (dqkv, dwq, dbq, dwk, dbk, colsum[2D]) like ``torch_ops.qk_norm_bwd``."""
     acc = torch.zeros(4 * hd + 2 * H * hd, dtype=torch.float32, device=qkv.device)
     dwq, dbq, dwk, dbk = acc[:4 * hd].view(4, hd)
     cs = acc[4 * hd:]
-    _C.qk_norm_bwd(dqkv, qkv, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, cs, H, hd)
+    if rope is None:
+        _C.qk_norm_bwd(dqkv, qkv, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, cs, H, hd)
+    else:
+        cos, sin, B, P, keep = rope
+        _C.qk_norm_rope_bwd(dqkv, qkv, wq, wk, mean, rstd, dwq, dbq, dwk, dbk, cs, cos, sin, keep, int(B), int(P), H,
+                            hd)
     return dqkv, dwq, dbq, dwk, dbk, cs
+
+
+# ------------------------------------------------------------------------------------------------
+# Rotary position embedding (csrc/rope.cu): 2-D axial RoPE on the q / k heads of the packed qkv buffer
+# ------------------------------------------------------------------------------------------------
+def rope_fwd(qkv, H: int, hd: int, cos, sin, B: int, P: int, keep=None, inplace: bool = False):
+    """out[:, 0:2D) = R qkv[:, 0:2D) like ``torch_ops.rope_fwd``; out of place, v and the prefix rows are copied."""
+    out = qkv if inplace else torch.empty(qkv.shape[0], 3 * H * hd, dtype=qkv.dtype, device=qkv.device)
+    _C.rope_fwd(qkv, out, cos, sin, keep, int(B), int(P), H, hd)
+    return out
+
+
+def rope_bwd(dqkv, H: int, hd: int, cos, sin, B: int, P: int, keep=None):
+    """In place on dqkv[:, 0:2D); returns (dqkv, colsum[2D]) like ``torch_ops.rope_bwd``."""
+    cs = torch.zeros(2 * H * hd, dtype=torch.float32, device=dqkv.device)
+    _C.rope_bwd(dqkv, cos, sin, keep, cs, int(B), int(P), H, hd)
+    return dqkv, cs
 
 
 # ------------------------------------------------------------------------------------------------

@@ -55,29 +55,37 @@ def ln_bwd(dy, x, w, mean, rstd, dres=None, want_dxsum: bool = False):
 # QK normalisation (timm Attention(qk_norm=True): q_norm / k_norm = nn.LayerNorm(head_dim) applied per head)
 # qkv is the packed [T, 3D] projection (D = H * hd); statistics are indexed [T, 2, H] (q heads, then k heads).
 # ------------------------------------------------------------------------------------------------
-def qk_norm_fwd(qkv, H: int, hd: int, wq, bq, wk, bk, eps: float, inplace: bool = False):
+def qk_norm_fwd(qkv, H: int, hd: int, wq, bq, wk, bk, eps: float, inplace: bool = False, rope=None):
     """Returns (out, mean, rstd): out = qkv with every q head normalised over hd (weight wq, bias bq) and every k head
-    (wk, bk), v unchanged; mean / rstd fp32 [T * 2 * H].  inplace=True writes into qkv itself and returns it."""
+    (wk, bk), v unchanged; mean / rstd fp32 [T * 2 * H].  inplace=True writes into qkv itself and returns it.
+    rope = (cos, sin, B, P, keep): the normalised q / k are then rotated like ``rope_fwd`` before the one rounding."""
     T, D = qkv.shape[0], H * hd
     x = _f32(qkv[:, : 2 * D]).reshape(T, 2, H, hd)
     mean = x.mean(dim=-1)
     rstd = torch.rsqrt(x.var(dim=-1, unbiased=False) + eps)
     w = torch.stack([_f32(wq), _f32(wk)])[None, :, None, :]
     b = torch.stack([_f32(bq), _f32(bk)])[None, :, None, :]
-    y = ((x - mean[..., None]) * rstd[..., None] * w + b).reshape(T, 2 * D).to(qkv.dtype)
+    y = ((x - mean[..., None]) * rstd[..., None] * w + b).reshape(T, 2 * D)
+    if rope is not None:
+        y = _rope_rotate(y, *rope, transpose=False)
+    y = y.to(qkv.dtype)
     out = qkv if inplace else qkv.clone()
     out[:, : 2 * D] = y
     return out, mean.reshape(-1), rstd.reshape(-1)
 
 
-def qk_norm_bwd(dqkv, qkv, H: int, hd: int, wq, wk, mean, rstd):
+def qk_norm_bwd(dqkv, qkv, H: int, hd: int, wq, wk, mean, rstd, rope=None):
     """LayerNorm backward of the q / k heads, in place on dqkv[:, 0:2D) (gradient of the normalised q / k in, of the
     un-normalised q / k out; dv untouched).  Returns (dqkv, dwq, dbq, dwk, dbk, colsum): fp32 [hd] parameter
     gradients summed over all T * H heads of each side, and fp32 [2D] column sums of the new (rounded) dq / dk, which
-    are the q / k part of the qkv bias gradient."""
+    are the q / k part of the qkv bias gradient.  rope = (cos, sin, B, P, keep): dq / dk are the gradients of the
+    rotated values and go through R^T, in fp32, first."""
     T, D = qkv.shape[0], H * hd
     x = _f32(qkv[:, : 2 * D]).reshape(T, 2, H, hd)
-    dy = _f32(dqkv[:, : 2 * D]).reshape(T, 2, H, hd)
+    dy = _f32(dqkv[:, : 2 * D])
+    if rope is not None:
+        dy = _rope_rotate(dy, *rope, transpose=True)
+    dy = dy.reshape(T, 2, H, hd)
     m, r = mean.view(T, 2, H, 1), rstd.view(T, 2, H, 1)
     xhat = (x - m) * r
     g = dy * torch.stack([_f32(wq), _f32(wk)])[None, :, None, :]
@@ -87,6 +95,47 @@ def qk_norm_bwd(dqkv, qkv, H: int, hd: int, wq, wk, mean, rstd):
     dqkv[:, : 2 * D] = dx.reshape(T, 2 * D).to(dqkv.dtype)
     cs = _f32(dqkv[:, : 2 * D]).sum(dim=0)
     return dqkv, dw[0], db[0], dw[1], db[1], cs
+
+
+# ------------------------------------------------------------------------------------------------
+# Rotary position embedding (2-D axial RoPE, EVA-02 / timm RotaryEmbeddingCat) on the q / k heads of the packed qkv
+# buffer of B images of T tokens.  Pair i of a head is its interleaved elements (2i, 2i + 1), rotated by the angle of
+# the fp32 tables cos / sin [N, hd / 2] (``vit.rope_tables``) at the token's patch: y0 = x0 c - x1 s, y1 = x1 c + x0 s.
+# Token j < P (class / register) is not rotated; patch token j uses table row keep[b, j - P], or j - P without keep.
+# ------------------------------------------------------------------------------------------------
+def _rope_rotate(x, cos, sin, B: int, P: int, keep, transpose: bool):
+    """fp32 [B * T, W] (W a whole number of heads) -> R x, or R^T x; the prefix rows are copied."""
+    rows, W = x.shape
+    T, half = rows // B, cos.shape[1]
+    idx = keep.long() if keep is not None else torch.arange(T - P, device=x.device).expand(B, T - P)
+    c = _f32(cos).to(x.device)[idx].unsqueeze(2)  # [B, K, 1, hd / 2]
+    s = _f32(sin).to(x.device)[idx].unsqueeze(2)
+    if transpose:
+        s = -s
+    xp = x.view(B, T, W // (2 * half), half, 2)[:, P:]
+    x0, x1 = xp[..., 0], xp[..., 1]
+    y = x.clone()
+    y.view(B, T, W // (2 * half), half, 2)[:, P:] = torch.stack((x0 * c - x1 * s, x1 * c + x0 * s), dim=-1)
+    return y
+
+
+def rope_fwd(qkv, H: int, hd: int, cos, sin, B: int, P: int, keep=None, inplace: bool = False):
+    """out[:, 0:2D) = R qkv[:, 0:2D) in fp32, rounded once; v and the prefix rows are copied bit for bit.
+    inplace=True writes into qkv itself and returns it."""
+    D = H * hd
+    y = _rope_rotate(_f32(qkv[:, : 2 * D]), cos, sin, B, P, keep, transpose=False).to(qkv.dtype)
+    out = qkv if inplace else qkv.clone()
+    out[:, : 2 * D] = y
+    return out
+
+
+def rope_bwd(dqkv, H: int, hd: int, cos, sin, B: int, P: int, keep=None):
+    """In place on dqkv[:, 0:2D): dq / dk become R^T dq / R^T dk (dv untouched).  Returns (dqkv, colsum): fp32 [2D]
+    column sums of the new (rounded) dq / dk, prefix rows included, which are the q / k part of the qkv bias
+    gradient (the attention backward's sums are those of the rotated gradient)."""
+    D = H * hd
+    dqkv[:, : 2 * D] = _rope_rotate(_f32(dqkv[:, : 2 * D]), cos, sin, B, P, keep, transpose=True).to(dqkv.dtype)
+    return dqkv, _f32(dqkv[:, : 2 * D]).sum(dim=0)
 
 
 # ------------------------------------------------------------------------------------------------

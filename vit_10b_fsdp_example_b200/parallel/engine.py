@@ -133,6 +133,7 @@ class FSDPViT:
         self._sumsq = None
         self._fused_sumsq = False
         self.step_count = 0        # optimizer steps since the start of training (checkpointed: seeds the dropout masks)
+        self._rope_tables = {}     # (image size, device) -> RoPE cos / sin; stable pointers for --cuda_graph
         self._steps_here = 0       # forward_backward calls of THIS process (the keep policy is sized after the first one)
         # All-gather fused into the qkv / fc1 GEMMs (copier warp pulling peer slabs with SM-issued loads): on by default
         # at W = 2 only; with more peers one warp per CTA has to pull (W - 1) / W of the weight while the GEMM waits
@@ -548,6 +549,20 @@ class FSDPViT:
         # g is [T, mlp_out_dim]: mlp_ratio units, or mlp_ratio / 2 with SwiGLU (the lean set's u is [T, Hd] either way)
         return (("P", p_bytes), ("h", 2 * unit), ("g", int(cfg.mlp_out_dim / cfg.embed_dim * unit)))
 
+    def _rope(self, stem_saved) -> dict:
+        """The ``rope=`` keyword of the block calls: {} without --rope (the calls stay as they were); otherwise the
+        tables, built once per (image size, device) so their pointers stay fixed under CUDA-graph replay, the prefix
+        length and, after patch dropout, the kept patches' original indices."""
+        cfg = self.cfg
+        if not cfg.rope:
+            return {}
+        key = (cfg.image_size, str(self.device))
+        if key not in self._rope_tables:
+            cos, sin = vit.rope_tables(cfg.grid, cfg.head_dim, cfg.rope_theta, cfg.rope_ref_grid)
+            self._rope_tables[key] = (cos.to(self.device), sin.to(self.device))
+        cos, sin = self._rope_tables[key]
+        return {"rope": vit.Rope(cos, sin, cfg.num_prefix_tokens, stem_saved.get("keep"))}
+
     def _save_mode(self, i: int, keep_from: int):
         """What block i stores in forward: False = only its input (checkpoint), True = everything
         (--no_grad_ckpt), else the set of extras kept on top of the lean set."""
@@ -599,6 +614,7 @@ class FSDPViT:
         self._wait_gather(self.root)
         rp = self.root.layout.param_views(self.root.full)
         x, stem_saved = vit.stem_forward(ops, cfg, rp, images, self.dtype, self.drop, mix=mix)
+        rope = self._rope(stem_saved)
         ckpt: List[torch.Tensor] = []
         saved_all = []
         for i, u in enumerate(blocks):
@@ -609,10 +625,10 @@ class FSDPViT:
             with self._range(f"fwd block {i}"):
                 if i < keep_from:
                     ckpt.append(x)
-                    x, _ = vit.block_forward(ops, cfg, p, x, B, save=False, drop=self.drop, block_idx=i)
+                    x, _ = vit.block_forward(ops, cfg, p, x, B, save=False, drop=self.drop, block_idx=i, **rope)
                 else:
                     x, s = vit.block_forward(ops, cfg, p, x, B, save=self._save_mode(i, keep_from), drop=self.drop,
-                                             block_idx=i)
+                                             block_idx=i, **rope)
                     saved_all.append(s)
             if self.reshard_after_forward and i != len(blocks) - 1:
                 self._release_params(u)  # the last block is needed again immediately by backward
@@ -633,11 +649,11 @@ class FSDPViT:
             with self._range(f"bwd block {i}"):
                 if i < keep_from:
                     xin = ckpt.pop()
-                    _, s = vit.block_forward(ops, cfg, p, xin, B, save=True, drop=self.drop, block_idx=i)
+                    _, s = vit.block_forward(ops, cfg, p, xin, B, save=True, drop=self.drop, block_idx=i, **rope)
                 else:
                     s = saved_all.pop()
                 g = self._grad_views(u)
-                dx, dx_sum = vit.block_backward(ops, cfg, p, g, s, dx, dx_sum, B)
+                dx, dx_sum = vit.block_backward(ops, cfg, p, g, s, dx, dx_sum, B, **rope)
                 del s
             self._release_params(u)
             self._issue_reduce(u)
@@ -668,12 +684,13 @@ class FSDPViT:
         rp = self.root.layout.param_views(self.root.full)
         drop = self.drop if self.training else None
         self.drop.sample_offset = self.rank * B
-        x, _ = vit.stem_forward(ops, cfg, rp, images, self.dtype, drop)
+        x, stem_saved = vit.stem_forward(ops, cfg, rp, images, self.dtype, drop)
+        rope = self._rope(stem_saved)
         for i, u in enumerate(blocks):
             if i + 1 < len(blocks):
                 self._issue_gather(blocks[i + 1], fuse=True)
             self._wait_gather(u)
-            x, _ = vit.block_forward(ops, cfg, self._views(u), x, B, save=False, drop=drop, block_idx=i)
+            x, _ = vit.block_forward(ops, cfg, self._views(u), x, B, save=False, drop=drop, block_idx=i, **rope)
             self._release_params(u)
         logits, _ = vit.head_forward(ops, cfg, rp, x, B)
         self.root.gather_event = None

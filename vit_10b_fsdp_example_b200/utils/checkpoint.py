@@ -3,7 +3,9 @@
 Layout kept compatible with the reference: one ``torch.save`` file per rank per epoch named
 ``epoch_{E}_rank_{R}.ckpt`` holding exactly four keys -- ``model`` (this rank's shards), ``shard_metadata``
 (``None`` when not FSDP), ``optimizer`` and ``lr_scheduler`` -- plus a fifth, ``model_ema`` (this rank's EMA shards,
-same layout as ``model``), only when the model keeps an EMA (``--model_ema``).  Every rank writes its own file; loading
+same layout as ``model``), only when the model keeps an EMA (``--model_ema``), and a sixth, ``rope`` (the
+``rope`` / ``rope_theta`` / ``rope_ref_grid`` settings), only with ``--rope``: the rotary embedding has no parameters,
+so only this record tells a resumed run how the weights were trained; a checkpoint without it had no RoPE.  Every rank writes its own file; loading
 goes through the host (``map_location='cpu'``).  ``consolidate_sharded_ckpts`` rebuilds a full state_dict.
 """
 from __future__ import annotations
@@ -24,6 +26,9 @@ def save_ckpt(ckpt_path: str, model, optimizer, lr_scheduler, master_only: bool 
     }
     if getattr(model, "has_ema", False):
         ckpt["model_ema"] = model.ema_state_dict()
+    rope = rope_settings(getattr(model, "cfg", None))
+    if rope is not None:
+        ckpt["rope"] = rope
     if not master_only or rank == 0:
         os.makedirs(os.path.dirname(os.path.abspath(ckpt_path)), exist_ok=True)
         tmp = ckpt_path + ".tmp"
@@ -34,9 +39,31 @@ def save_ckpt(ckpt_path: str, model, optimizer, lr_scheduler, master_only: bool 
     print(f"checkpoint saved to {ckpt_path}\n", end="")
 
 
+def rope_settings(cfg):
+    """The RoPE record of a checkpoint: {"rope": True, "rope_theta": .., "rope_ref_grid": ..}, or None without RoPE."""
+    if cfg is None or not getattr(cfg, "rope", False):
+        return None
+    return {"rope": True, "rope_theta": float(cfg.rope_theta), "rope_ref_grid": int(cfg.rope_ref_grid)}
+
+
+def check_rope_settings(saved, cfg, ckpt_path: str) -> None:
+    """Refuses to resume weights trained under other RoPE settings, naming the flags that would match them."""
+    want = rope_settings(cfg)
+    if saved == want:
+        return
+    if saved is None:
+        fix = "drop --rope, --rope_theta and --rope_ref_grid"
+    else:
+        fix = f"pass --rope --rope_theta {saved['rope_theta']:g} --rope_ref_grid {saved['rope_ref_grid']}"
+    raise ValueError(f"checkpoint {ckpt_path} was trained with rotary position embedding settings {saved or 'no RoPE'}, "
+                     f"this run has {want or 'no RoPE'}: {fix} to resume it")
+
+
 def load_ckpt(ckpt_path: str, model, optimizer, lr_scheduler) -> None:
     assert os.path.exists(ckpt_path), f"checkpoint {ckpt_path} does not exist"
     ckpt = torch.load(ckpt_path, map_location="cpu", weights_only=False)
+    if hasattr(model, "cfg"):
+        check_rope_settings(ckpt.get("rope"), model.cfg, ckpt_path)
     try:
         model.load_state_dict(ckpt["model"], shard_metadata=ckpt.get("shard_metadata"))
     except TypeError:  # a plain nn.Module-style model
